@@ -20,8 +20,13 @@ configs[3] at its stated length (50 waypoints, CartVel + LVS continuous collisio
 Every step uses a different synthetic batch (seed = f(step, rank)), so nothing is cached between timed iterations; the
 working set of one step (~0.6 GB of convexification rows + QP workspace at B=1024 with collision) is larger than L2.
 --scaling strong splits ONE global batch (--batch) over the ranks instead of giving every rank its own.
+--dump-outputs DIR writes the results of the last timed step of the resident leg on rank 0 (what tb200_fetch_results
+hands a caller) as DIR/<name>.npy in float64, so that two builds can be compared output for output on the same seeded
+inputs.  Above DUMP_LIMIT bytes in all, a fixed seeded sample of the trajectories is written instead, with its indices
+in DIR/trajectory_index.npy.
 """
 import argparse
+import atexit
 import json
 import os
 import subprocess
@@ -80,7 +85,7 @@ def config_dict(args, world):
 # ---------------------------------------------------------------------------------------------------------- host info
 def host_info():
     """What the CPU arm runs on: logical CPUs, physical cores, the CPUs this process may use, the cgroup CPU quota,
-    the CPU model and the load when the measurement starts (two boxes of one pool have differed 3.5x in round 1)."""
+    the CPU model and the load when the measurement starts (CPU numbers of two hosts are only comparable with these)."""
     info = {"logical_cpus": os.cpu_count()}
     try:
         info["affinity"] = len(os.sched_getaffinity(0))
@@ -113,9 +118,8 @@ def host_info():
 
 def host_threads(info=None):
     """Host threads of the CPU legs: one per physical core this process may run on, capped by the cgroup CPU quota
-    (torchrun exports OMP_NUM_THREADS=1, which must not shrink the CPU baseline).  Measured on the GPU box in round 1
-    (2 x 64 hardware threads), full batch of 1024: 64 threads 6.3 s, 128 threads 8.5 s - the oracle is bound by its
-    allocator and caches, SMT siblings only hurt."""
+    (torchrun exports OMP_NUM_THREADS=1, which must not shrink the CPU baseline).  The oracle is bound by its allocator
+    and caches: SMT siblings only slow it down."""
     if os.environ.get("TB200_CPU_THREADS"):
         return int(os.environ["TB200_CPU_THREADS"])
     info = info or host_info()
@@ -130,7 +134,7 @@ def host_threads(info=None):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
 
     def __init__(self, index):
         self.index = index
@@ -144,6 +148,7 @@ class ClockSampler:
             self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader,nounits", "-i",
                                           str(self.index), "-lms", "100"], stdout=subprocess.PIPE, text=True)
             threading.Thread(target=self._read, daemon=True).start()
+            atexit.register(self._kill)  # never outlive bench.py, whatever ends it
         except OSError:
             self.proc = None
 
@@ -151,10 +156,15 @@ class ClockSampler:
         for line in self.proc.stdout:
             self.samples.append([c.strip() for c in line.split(",")])
 
+    def _kill(self):
+        if self.proc is not None and self.proc.poll() is None:
+            self.proc.terminate()
+            self.proc.wait()
+
     def stop(self):
         if self.proc is None:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
-        self.proc.terminate()
+        self._kill()
         sm = [float(s[0]) for s in self.samples if s and s[0].replace(".", "").isdigit()]
         mx = [float(s[1]) for s in self.samples if len(s) > 1 and s[1].replace(".", "").isdigit()]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
@@ -184,7 +194,7 @@ def cpu_time(oracle_lib, desc, threads, b1=None, repeats=1):
 
 
 def cpu_sweep(oracle_lib, desc, threads):
-    """Thread scaling of the CPU path on a small sample (explains the quoted number: does the box deliver its cores?)
+    """Thread scaling of the CPU path on a small sample (explains the quoted number: does the host deliver its cores?)
     and the single-thread latency per trajectory."""
     out = {}
     t1, _ = cpu_time(oracle_lib, desc, 1, b1=min(16, desc.B))
@@ -234,14 +244,35 @@ def run_reference(args, rank, world):
 
 # ----------------------------------------------------------------------------------------------------------- CUDA arm
 def measured_traffic(config):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one full-batch convexify launch from this round's
-    `ncu --set full` capture (profiles/r02_convexify_ncu.json, written by scripts/ncu_traffic.py); None without one."""
-    path = os.path.join(ROOT, "profiles", "r02_convexify_ncu.json")
+    """dram__bytes_read.sum + dram__bytes_write.sum of one full-batch convexify launch from an `ncu --set full` capture
+    (profiles/convexify_ncu.json, written by scripts/ncu_traffic.py); None without one."""
+    path = os.path.join(ROOT, "profiles", "convexify_ncu.json")
     try:
         d = json.load(open(path))
         return d.get(config, {}).get("dram_bytes")
     except (OSError, ValueError):
         return None
+
+
+DUMP_LIMIT = 64 * 10**6  # bytes of all dumped files together
+DUMP_KEYS = ("x", "status", "total_cost", "cost_vals", "cnt_viols", "n_qp_solves", "n_func_evals", "n_admm_iters")
+
+
+def dump_outputs(out_dir, res):
+    """The result arrays of one solve as <name>.npy, float64 (integer counters and status codes are exact in it).  Every
+    array is indexed by trajectory first; when they exceed DUMP_LIMIT together, the same seeded sample of trajectories
+    is taken from each, and trajectory_index.npy names it."""
+    os.makedirs(out_dir, exist_ok=True)
+    B = len(res["status"])
+    per_traj = sum(8 * res[k][0].size for k in DUMP_KEYS) + 8
+    idx = None
+    if B * per_traj > DUMP_LIMIT:
+        room = DUMP_LIMIT - 256 * (len(DUMP_KEYS) + 1)  # less the .npy headers
+        idx = np.sort(np.random.default_rng(0).choice(B, room // per_traj, replace=False))
+        np.save(os.path.join(out_dir, "trajectory_index.npy"), idx.astype(np.float64))
+    for k in DUMP_KEYS:
+        a = res[k] if idx is None else res[k][idx]
+        np.save(os.path.join(out_dir, k + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
 
 
 def main():
@@ -260,7 +291,11 @@ def main():
     ap.add_argument("--cpu-repeats", type=int, default=3, help="cpu_baseline: best of this many runs")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the results of the last timed resident step (rank 0) to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if args.batch <= 0:
         args.batch = DEFAULT_BATCH[args.config]
 
@@ -339,10 +374,10 @@ def main():
     t0 = time.perf_counter()
     e2e_conv, h2d, d2h, last = 0, 0, 0, None
     for it in range(args.warmup, total):
-        res = step_e2e(it)
-        e2e_conv += int((res["status"] == 0).sum())
-        h2d, d2h = res["timing"]["h2d_bytes"], res["timing"]["d2h_bytes"]
-        last = res
+        out = step_e2e(it)
+        e2e_conv += int((out["status"] == 0).sum())
+        h2d, d2h = out["timing"]["h2d_bytes"], out["timing"]["d2h_bytes"]
+        last = out
     torch.cuda.synchronize()
     e2e_s = time.perf_counter() - t0
     clocks = sampler.stop() if rank == 0 else None
@@ -363,6 +398,8 @@ def main():
     # the batches of every rank, step by step: a batch is as slow as its longest trajectory (tens of thousands of
     # dependent ADMM iterations), so its time varies with the draw — the spread is part of the measurement
     step_ms_min, step_ms_max = reduce(-min(dev_ms), MAX), reduce(max(dev_ms), MAX)
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, res)  # the resident leg's last step: the one `value` is measured on
     if rank != 0:
         if world > 1:
             dist.destroy_process_group()
@@ -371,7 +408,7 @@ def main():
     value = conv_total / dev_total_s
     # ---- roofline of the convexify kernel (HBM bound; algorithmic bytes per launch: DESIGN.md section 4) -------------
     peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+    peak, peak_src = 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (burst)"
     conv_ms = sum(t["convexify_ms"] for t in tms)
@@ -402,7 +439,7 @@ def main():
             "gpu_launches": 4 * len(tms) + 3 * args.steps,
             "roofline": roofline,
             "qp_steps": {"share_of_step": qp_ms / sum(dev_ms), "qp_solves": int(sum(t["qp_launches"] for t in tms)),
-                         "note": "QP steps of solve_kernel (ADMM): shared-memory/latency bound, see profiles/ for achieved occupancy"},
+                         "note": "QP steps of solve_kernel (ADMM): shared-memory/latency bound"},
             "clocks": clocks}
     oracle_lib = None
     if not args.no_parity:

@@ -1,5 +1,5 @@
 /*
- * trajopt_b200.h — C ABI of the B200-native batched SQP trajectory optimizer.
+ * trajopt_b200.h — C ABI of the H100-native (sm_90a) batched SQP trajectory optimizer.
  *
  * This header is the drop-in boundary for ONE path of tesseract-robotics/trajopt:
  * sco::BasicTrustRegionSQP::optimize() (trajopt_sco/src/optimizers.cpp:699-991) with its

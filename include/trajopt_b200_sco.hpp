@@ -3,7 +3,7 @@
 // Mirrors trajopt_sco/include/trajopt_sco/solver_interface.hpp:40-290 by name: sco::Var / Cnt / AffExpr / QuadExpr,
 // sco::Model with addVar / addEqCnt / addIneqCnt / removeVars / removeCnts / update / setVarBounds / setObjective /
 // optimize / getVarValues / writeToFile / getVars, sco::ModelType, sco::createModel(ModelType).  A caller of the
-// reference's sco layer (its BasicTrustRegionSQP, or any code that builds QPs through sco::Model) gets the B200 QP
+// reference's sco layer (its BasicTrustRegionSQP, or any code that builds QPs through sco::Model) gets the GPU QP
 // solver as its back end by including this header and linking libtrajopt_b200.so: createModel() returns a model whose
 // optimize() assembles OSQP's canonical form exactly as OSQPModel does (osqp_interface.cpp:170-281: P = M + M', upper
 // triangle; A = [constraint rows; I]; EQ rows before nothing in particular — row order is insertion order) and hands it to
@@ -218,7 +218,7 @@ struct ModelConfig {
   using ConstPtr = std::shared_ptr<const ModelConfig>;
   virtual ~ModelConfig() = default;
 };
-// settings of the B200 QP back end (the OSQPModelConfig of this library: osqp_interface.hpp:17-36)
+// settings of the GPU QP back end (the OSQPModelConfig of this library: osqp_interface.hpp:17-36)
 struct B200ModelConfig : ModelConfig {
   tb200_qp_settings settings;
   int device = 0;

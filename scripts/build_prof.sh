@@ -4,12 +4,12 @@
 # Used by scripts/prof_phases.py and scripts/eval_phases.py through TB200_LIB=<path>.
 set -e
 cd "$(dirname "$0")/../trajopt_b200/csrc"
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -ccbin /usr/bin/g++"
+FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -ccbin /usr/bin/g++"
 nvcc $FLAGS -DTB200_PROFILE $PROF_EXTRA -c -o solve_inst_7_0.prof.o solve_inst_7_0.cu &
 nvcc $FLAGS -DTB200_PROFILE -c -o solve_inst_7_1.prof.o solve_inst_7_1.cu &
 nvcc $FLAGS -DTB200_EVAL_PROFILE -c -o eval_kernels.prof.o eval_kernels.cu &
 wait
 OBJS=$(ls *.o | grep -v '\.prof\.o$' | grep -v '^solve_inst_7_[01]\.o$' | grep -v '^eval_kernels\.o$')
-nvcc -shared -gencode arch=compute_100a,code=sm_100a -ccbin /usr/bin/g++ -o libtb200_prof.so $OBJS solve_inst_7_0.prof.o solve_inst_7_1.prof.o eval_kernels.prof.o
+nvcc -shared -gencode arch=compute_90a,code=sm_90a -ccbin /usr/bin/g++ -o libtb200_prof.so $OBJS solve_inst_7_0.prof.o solve_inst_7_1.prof.o eval_kernels.prof.o
 rm -f solve_inst_7_0.prof.o solve_inst_7_1.prof.o eval_kernels.prof.o
 echo built libtb200_prof.so

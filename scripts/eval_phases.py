@@ -29,7 +29,8 @@ st, en, smid = (tr[:, 0] - t0) * 1e-3, (tr[:, 1] - t0) * 1e-3, tr[:, 2].astype(i
 dur = en - st
 print(f"timeline: first start 0, last end {en.max():.1f} us; CTA duration us: mean {dur.mean():.1f} p10 {np.percentile(dur,10):.1f} p50 {np.percentile(dur,50):.1f} p90 {np.percentile(dur,90):.1f} max {dur.max():.1f}")
 print("CTA starts (us) percentiles:", " ".join(f"p{q}={np.percentile(st,q):.1f}" for q in (1, 25, 50, 58, 60, 75, 99)))
-per_sm = np.bincount(smid, minlength=148)
+import torch
+per_sm = np.bincount(smid, minlength=torch.cuda.get_device_properties(0).multi_processor_count)
 print("CTAs per SM: min", per_sm.min(), "max", per_sm.max(), "SMs used", (per_sm > 0).sum())
 grid = np.linspace(0, en.max(), 21)
 print("resident CTAs over time:", " ".join(f"{((st <= g) & (en > g)).sum()}" for g in grid))

@@ -1,5 +1,6 @@
 """Extracts duration / DRAM traffic / key metrics of one kernel from an `ncu --set full` report into a small JSON under
-profiles/ (bench.py reads roofline.traffic from it).  usage: ncu_traffic.py report.ncu-rep cfg2 out.json"""
+profiles/ (bench.py reads roofline.traffic from profiles/convexify_ncu.json).
+usage: ncu_traffic.py report.ncu-rep cfg2 profiles/convexify_ncu.json"""
 import csv
 import io
 import json

@@ -1,6 +1,6 @@
 // Latency probe for the building blocks of one ADMM iteration (one CTA of 256 threads on one SM):
 // dependent DFMA chain, 64-bit shuffle, LDS.128, __syncthreads with 8 warps, and one block-cyclic-reduction level
-// (7 x LDS.128 + 14 DFMA in two chains + shuffle + STS + barrier).  nvcc -arch=sm_100a -O3 lat_probe.cu -o lat_probe
+// (7 x LDS.128 + 14 DFMA in two chains + shuffle + STS + barrier).  nvcc -arch=sm_90a -O3 lat_probe.cu -o lat_probe
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -17,7 +17,9 @@ t0 = float(buf[0]); fin = (buf[1:1 + B].astype(np.float64) - t0) * 1e-6; busy = 
 it = got["n_admm_iters"].astype(np.float64)
 print(f"{cfg} B={B}: total {tm['total_ms']:.1f} ms; converged {(got['status'] == 0).sum()}; ADMM iterations {it.sum():.0f} (max {it.max():.0f})")
 print("finish time percentiles (ms): " + " ".join(f"p{q}={np.percentile(fin, q):.0f}" for q in (10, 50, 90, 99, 100)))
-print(f"SM busy time {busy.sum():.0f} ms = {busy.sum() / (148 * fin.max()) * 100:.0f}% of 148 SMs x {fin.max():.0f} ms; ns per ADMM iteration (busy / iterations): {busy.sum() * 1e6 / it.sum():.0f}")
+import torch
+n_sm = torch.cuda.get_device_properties(0).multi_processor_count
+print(f"SM busy time {busy.sum():.0f} ms = {busy.sum() / (n_sm * fin.max()) * 100:.0f}% of {n_sm} SMs x {fin.max():.0f} ms; ns per ADMM iteration (busy / iterations): {busy.sum() * 1e6 / it.sum():.0f}")
 last = np.argsort(-fin)[:8]
 for b in last:
     print(f"  traj {b}: finished {fin[b]:.0f} ms, busy {busy[b]:.0f} ms ({100 * busy[b] / fin[b]:.0f}% of its life), {it[b]:.0f} iterations, {got['n_qp_solves'][b]} QPs, status {got['status'][b]}")

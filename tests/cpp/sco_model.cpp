@@ -45,7 +45,7 @@ static double exprMultCase(double v1_val, double v2_val, double v1_coeff, double
   const QuadExpr aff12 = exprMult(aff1, aff2);
   solver->setObjective(aff12);
   solver->update();
-  solver->writeToFile("/tmp/solver-interface-test.lp");
+  solver->writeToFile("solver-interface-test.lp");  // in the working directory the test gives
   solver->optimize();
   DblVec soln(2);
   for (std::size_t i = 0; i < 2; ++i) soln[i] = solver->getVarValue(vars[i]);

@@ -1,4 +1,4 @@
-"""CPU-only checks of the C-ABI boundary: the CUDA library builds for sm_100a, loads without a GPU and
+"""CPU-only checks of the C-ABI boundary: the CUDA library builds for sm_90a, loads without a GPU and
 exports every symbol include/trajopt_b200.h declares; the product fails loudly (never falls back) when no
 device is present."""
 import ctypes as C

@@ -45,8 +45,8 @@ def test_model_assembles_the_canonical_qp(exe):
 
 
 @pytest.mark.gpu
-def test_reference_solver_interface_cases(exe):
-    out = subprocess.run([exe, "solve"], check=True, capture_output=True, text=True).stdout
+def test_reference_solver_interface_cases(exe, tmp_path):
+    out = subprocess.run([exe, "solve"], check=True, capture_output=True, text=True, cwd=tmp_path).stdout
     lines = {l.split()[0]: l.split() for l in out.strip().split("\n")}
     assert lines["setup_problem"][2] == "0" and abs(float(lines["setup_problem"][4])) < 1e-6, out  # EXPECT_NEAR(aff.value, 0, 1e-6)
     assert lines["vars_after_remove"][1] == "2"

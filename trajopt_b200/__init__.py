@@ -1,1 +1,1 @@
-"""trajopt_b200 — B200-native batched SQP trajectory optimizer (hot path of tesseract-robotics/trajopt)."""
+"""trajopt_b200 — H100-native (sm_90a) batched SQP trajectory optimizer (hot path of tesseract-robotics/trajopt)."""

@@ -1,4 +1,4 @@
-// Device-side data model of the batched SQP hot path (sm_100a).  See DESIGN.md §3 for the HBM layout.
+// Device-side data model of the batched SQP hot path (sm_90a).  See DESIGN.md §3 for the HBM layout.
 #pragma once
 #include <cstdint>
 

@@ -584,8 +584,8 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
               // rows are 16-byte aligned (D + 3 even, 256-byte aligned buffers): the 32 rows of the chunk are staged in
               // shared memory and leave as warp-contiguous 16-byte stores (512 contiguous bytes per store instruction,
               // 2.5 KB contiguous per chunk).  (A cp.async.bulk store of the tile moves the same bytes, but the tile can
-              // only be refilled once the bulk engine has read it — microseconds with 24 warps per SM queueing their
-              // stores — and the row phase of a CTA took 32k cycles; plain stores are fire and forget.)
+              // only be refilled once the bulk engine has read it, which serialises the row phase; plain stores are fire
+              // and forget.)
               if (in) {
                 double2* d2 = reinterpret_cast<double2*>(stage + lane_c * (D + 3));
 #pragma unroll
@@ -1001,6 +1001,9 @@ __device__ __noinline__ void eval_step(const DevProblem& p, const EvalExtra& ex,
   eval_step_impl<DD>(p, ex, mode, b, x_in, tables_ready);
 }
 
+// Two CTAs per SM cap the 7-joint instance at 128 registers, and on sm_90a ptxas spills a few of them; one CTA per SM
+// needs 180 and none spill.  Measured on an H100 (configs[2], full batch of 1024): 111-119 us per launch with two
+// CTAs per SM against 140-144 us with one, the same SQP throughput either way.  So two stay.
 #ifndef TB200_EVAL_MIN_BLOCKS
 #define TB200_EVAL_MIN_BLOCKS 2
 #endif
@@ -1011,7 +1014,7 @@ __global__ void __launch_bounds__(kEvalThreads, (DD <= 8) ? TB200_EVAL_MIN_BLOCK
 eval_convexify_decide_kernel(const __grid_constant__ DevProblem p, const __grid_constant__ EvalExtra ex, int mode,
                              const double* x_in /*EVAL_ONLY*/) {
   // persistent CTAs: the grid fills the SMs once and every CTA takes the next trajectory when it is done with one
-  // (1024 trajectories over 148 SMs x 3-4 resident CTAs: no tail wave of half-empty SMs)
+  // (1024 trajectories over 132 SMs x 2 resident CTAs: no tail wave of half-empty SMs)
   __shared__ int s_next;
   bool tables_ready = false;  // the robot / object tables stay in shared memory from one trajectory to the next
   for (;;) {

@@ -156,8 +156,8 @@ __host__ __device__ inline QpSmem qp_smem_layout(int N, int nb, int row_stride, 
   // the factor (SA, SLM, SU contiguous) when it fits, then the objective's band P(i, i-k), then rows with what is left
   // (bank layout: the solve reads SA and SU side by side in its backward tasks and SU and SLM side by side in its
   // forward tasks, even lanes one matrix, odd lanes the other: SLM starts a multiple of 16 doubles after SA and SU
-  // 8 doubles (16 banks) off that grid, so the two halves of a warp's access land on disjoint banks.  Measured before:
-  // 1.5 G bank conflicts in a 344 ms launch.)
+  // 8 doubles (16 banks) off that grid, so the two halves of a warp's access land on disjoint banks; before this layout
+  // bank conflicts dominated the solve.)
   const int fA = (M * blk + 15) & ~15, fL = fA + 8, fU = qp_even(M * blk);
   s.factor_smem = (!factor_global && o + fA + fL + fU <= kQpSmemBudget) ? 1 : 0;
   o = s.factor_smem ? ((o + 15) & ~15) : o;
@@ -888,9 +888,9 @@ __device__ __forceinline__ void bcr_solve_sm(const int tid, const SolveRoles& R,
 // Register-resident solve for the ADMM block (called with the whole register file at its disposal): every thread
 // applies the same few factor rows in every solve, so they live in registers (level 0: one forward and one backward
 // row; upper levels: one each for the threads that have a role there) and a level only reads the right-hand side —
-// a few distinct 16-byte words per warp — from shared memory.  Measured with the rows read from shared memory instead:
-// level 0 alone moves 44 KB (down) and 75 KB (up) per solve through the 128 B/clock shared-memory port, 210 KB per
-// solve in all = 1640 cycles of pure bandwidth.  The loads of a level are issued before its multiply-adds.
+// a few distinct 16-byte words per warp — from shared memory.  With the rows read from shared memory instead, level 0
+// alone would move 44 KB (down) and 75 KB (up) per solve through the 128 B/clock shared-memory port, 210 KB per solve
+// in all = 1640 cycles of pure bandwidth.  The loads of a level are issued before its multiply-adds.
 template <int NB>
 __device__ __forceinline__ double reg_fwd_task(const double (&m)[NB], const double* yv) {
   constexpr int H = NB / 2;
@@ -1249,8 +1249,8 @@ __device__ inline bool pinv_factor(const QpCtx& q) {
   }
   __syncthreads();
   // ---- 3. Schur complement on the separators: S = A_ss - C' W (block tridiagonal in the separators).  One entry per
-  // thread and pass; the dot products are unrolled with two partial sums each (a dependent chain of 28 multiply-adds
-  // with its loads in between took 1.3 k cycles per entry)
+  // thread and pass; the dot products are unrolled with two partial sums each (a single dependent chain of 28
+  // multiply-adds with its loads in between is bound by their latency)
   for (int e = tid; e < nS * nS; e += kQpThreads) {
     const int ra = e / nS, ca = e % nS, sa = ra / NB, i = ra % NB, sb = ca / NB, j = ca % NB;
     double v = 0.0;

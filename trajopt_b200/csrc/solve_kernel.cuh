@@ -11,8 +11,8 @@
 // what makes a trajectory long is slow ADMM convergence of its QPs, which shows from its first QPs on.  So the
 // ready trajectory with the highest mean ADMM iterations per QP so far runs first (not yet started ones before
 // all others): the long ones start early and run almost without interruption while the short ones fill the
-// remaining SMs.  Simulated on the measured per-QP iteration counts of configs[2]: 0.65 s against 0.78 s for
-// round robin and 1.15 s for lock-step launches (bound: 0.57 s, the longest trajectory alone).
+// remaining SMs.  An event-driven simulation on the per-QP iteration counts of configs[2] puts this order ahead of
+// round robin and of lock-step launches, and close to the bound set by the longest trajectory alone.
 //
 // Hand-over between CTAs goes through sched_state[b] (0 ready, 1 running, 2 finished): release = barrier, fence,
 // atomic store by thread 0; acquire = atomic CAS by thread 0, fence, barrier.

@@ -70,7 +70,7 @@ struct tb200_problem {
   tb200_layout layout{};
   int B = 0, T = 0, D = 0, N = 0;
   size_t eval_smem = 0, qp_smem = 0, solve_smem = 0;
-  int n_sm = 148;
+  int n_sm = 132;  // H100 SXM; replaced by the device's own count at problem creation
   int quantum = 3;  // SQP steps a CTA runs of a trajectory before it looks for a more urgent one (TB200_QUANTUM overrides)
   cudaStream_t stream = nullptr;
   tb200_timing timing{};
@@ -114,7 +114,7 @@ struct tb200_problem {
 
 extern "C" {
 
-const char* tb200_version(void) { return "trajopt_b200 0.1 (sm_100a)"; }
+const char* tb200_version(void) { return "trajopt_b200 0.1 (sm_90a)"; }
 const char* tb200_last_error(void) { return g_err.c_str(); }
 
 void tb200_default_sqp_params(tb200_sqp_params* p) {  // optimizers.hpp:92-135
