@@ -148,6 +148,7 @@ struct DevProblem {
   int* sched_state;            // [B] persistent SQP kernel: 0 ready, 1 running, 2 finished
   unsigned long long* sched_timers;  // [4] ns in QP steps, ns in evaluation steps, evaluation steps, claims
   QpSettings qp;
+  int qp_fast_passes;  // 1: short trajectories take the fused termination check and polish_passes (qp_cta_kernel.cuh)
   SqpParams sqp;
 };
 

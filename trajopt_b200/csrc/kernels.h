@@ -13,5 +13,6 @@ using EvalKernelFn = void (*)(DevProblem, EvalExtra, int, const double*);
 SolveKernelFn solve_kernel_for(int D, bool pair_rows);
 EvalKernelFn eval_kernel_for(int D);
 int eval_debug_prof(unsigned long long* out, int reset);  // TB200_EVAL_PROFILE builds of eval_kernels.cu only
-int qp_debug_prof(unsigned long long* out, int reset);  // TB200_PROFILE builds only (else returns -1)
+constexpr int kQpProfSlots = 32;  // phase counters of a TB200_PROFILE build (slot meanings: scripts/prof_phases.py)
+int qp_debug_prof(unsigned long long* out, int reset);  // out[kQpProfSlots]; TB200_PROFILE builds only (else returns -1)
 }  // namespace tb200

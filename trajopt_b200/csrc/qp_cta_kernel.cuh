@@ -39,12 +39,14 @@
 namespace tb200 {
 
 #ifdef TB200_PROFILE
-static __device__ unsigned long long g_prof[16];
+static __device__ unsigned long long g_prof[32];
 #define PROF_T0() const long long prof_t0_ = clock64()
 #define PROF_ADD(slot) do { if (q.tid == 0) atomicAdd(&g_prof[slot], (unsigned long long)(clock64() - prof_t0_)); } while (0)
+#define PROF_COUNT(slot) do { if (q.tid == 0) atomicAdd(&g_prof[slot], 1ull); } while (0)
 #else
 #define PROF_T0()
 #define PROF_ADD(slot)
+#define PROF_COUNT(slot)
 #endif
 // -DTB200_PROFILE_CHECK: the per-level slots of the solve (4, 14, 15, 9) count the parts of a termination check instead
 #if defined(TB200_PROFILE) && defined(TB200_PROFILE_CHECK)
@@ -1026,48 +1028,164 @@ __device__ __forceinline__ void bcr_solve_hyb(const int tid, const SolveRoles& R
 
 // scaled P (band) times a vector: out = c * Dz .* (P (Dz .* in)); in: shared or global, out: global/shared.
 // The band loads are independent and fully unrolled, so the pass costs one memory round trip, not 2*HB+1.
+// row i < N of that product; Dz and vin are shared-memory vectors
+template <int NB>
+__device__ __forceinline__ double p_row(const QpCtx& q, const int i, const double* Dz, const double* vin) {
+  constexpr int HB = NB, W = HB + 1;
+  const int N = q.N, nbo = q.n_band;
+  const double* const Pb = q.Pband;  // shared or global
+  const int* const offs = q.band_offs;
+  double s = 0.0;
+  // (P * Dz) and x, multiplied and added in the reference's order: the lower part of row i (k ascending), then the
+  // upper part; only the structurally non-zero offsets are visited (a skipped entry adds an exact zero)
+  for (int t0 = 0; t0 < nbo; t0 += 4) {
+    double v[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int k = (t0 + u < nbo) ? offs[t0 + u] : -1;
+      v[u] = (k >= 0 && k <= i) ? (Pb[i * W + k] * Dz[i - k]) * vin[i - k] : 0.0;
+    }
+    s += v[0]; s += v[1]; s += v[2]; s += v[3];
+  }
+  for (int t0 = 0; t0 < nbo; t0 += 4) {
+    double v[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int k = (t0 + u < nbo) ? offs[t0 + u] : -1;
+      v[u] = (k >= 1 && i + k < N) ? (Pb[(i + k) * W + k] * Dz[i + k]) * vin[i + k] : 0.0;
+    }
+    s += v[0]; s += v[1]; s += v[2]; s += v[3];
+  }
+  return s * (q.c * Dz[i]);
+}
 template <int NB>
 __device__ __forceinline__ void p_matvec(const QpCtx& q, const double* in, double* out) {
-  // in, out and the scalings are vectors of the CTA's shared memory: addressed as offsets (ld.shared); everything the
-  // loop needs is copied to locals first, and the band offsets are visited four at a time with their loads side by side
+  // in, out and the scalings are vectors of the CTA's shared memory: addressed as offsets (ld.shared); the band
+  // offsets are visited four at a time with their loads side by side
   extern __shared__ double sm[];
-  constexpr int HB = NB, W = HB + 1;
-  const int N = q.N, Np = q.Np, nbo = q.n_band;
-  const double* const Pb = q.Pband;  // shared or global
+  const int N = q.N, Np = q.Np;
   const double* const Dz = sm + (q.Dz - q.smbase);
   const double* const vin = sm + (in - q.smbase);
   double* const vout = sm + (out - q.smbase);
-  const int* const offs = q.band_offs;
-  const double cc = q.c;
-  for (int i = q.tid; i < Np; i += kQpThreads) {
-    double s = 0.0;
-    if (i < N) {
-      // (P * Dz) and x, multiplied and added in the reference's order: the lower part of row i (k ascending), then the
-      // upper part; only the structurally non-zero offsets are visited (a skipped entry adds an exact zero)
-      for (int t0 = 0; t0 < nbo; t0 += 4) {
-        double v[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const int k = (t0 + u < nbo) ? offs[t0 + u] : -1;
-          v[u] = (k >= 0 && k <= i) ? (Pb[i * W + k] * Dz[i - k]) * vin[i - k] : 0.0;
-        }
-        s += v[0]; s += v[1]; s += v[2]; s += v[3];
-      }
-      for (int t0 = 0; t0 < nbo; t0 += 4) {
-        double v[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const int k = (t0 + u < nbo) ? offs[t0 + u] : -1;
-          v[u] = (k >= 1 && i + k < N) ? (Pb[(i + k) * W + k] * Dz[i + k]) * vin[i + k] : 0.0;
-        }
-        s += v[0]; s += v[1]; s += v[2]; s += v[3];
-      }
-      s *= cc * Dz[i];
-    }
-    vout[i] = s;
-  }
+  for (int i = q.tid; i < Np; i += kQpThreads) vout[i] = (i < N) ? p_row<NB>(q, i, Dz, vin) : 0.0;
   __syncthreads();
 }
+
+// ---- the terms of a termination check, per row and per variable -------------------------------------------
+// Shared by the generic passes of qp_solve_block and the check fused into admm_block_pinv, so that both compute every
+// term with the same expression.  m[14]: 0 pri 1 z 2 ax 3 dua 4 aty 5 q 6 px | 7..13 the same on the scaled quantities.
+__device__ __forceinline__ void info_row_terms(const double* F, const double ax, double (&m)[14]) {
+  const double einv = 1.0 / F[R_E];
+  m[0] = fmax(m[0], fabs(einv * (ax - F[R_Z])));
+  m[1] = fmax(m[1], fabs(einv * F[R_Z]));
+  m[2] = fmax(m[2], fabs(einv * ax));
+  m[7] = fmax(m[7], fabs(ax - F[R_Z]));
+  m[8] = fmax(m[8], fabs(F[R_Z]));
+  m[9] = fmax(m[9], fabs(ax));
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {  // absent aux slots contribute exact zeros
+    const double u = F[R_U0 + k], bb = F[R_B0 + k], qa = F[R_QA0 + k];
+    const double xa = F[R_XA0 + k], za = F[R_ZA0 + k], ya = F[R_YA0 + k];
+    // Einv / Dinv of the aux row and column: one reciprocal each, multiplied like the Einv[r] * (...) of the oracle
+    const double iea = 1.0 / F[R_EA0 + k], ida = 1.0 / F[R_DA0 + k];
+    const double axb = bb * xa;
+    m[0] = fmax(m[0], fabs(iea * (axb - za)));
+    m[1] = fmax(m[1], fabs(iea * za));
+    m[2] = fmax(m[2], fabs(iea * axb));
+    m[7] = fmax(m[7], fabs(axb - za));
+    m[8] = fmax(m[8], fabs(za));
+    m[9] = fmax(m[9], fabs(axb));
+    const double aty = u * F[R_Y] + bb * ya;
+    m[3] = fmax(m[3], fabs(ida * (qa + aty)));
+    m[4] = fmax(m[4], fabs(ida * aty));
+    m[5] = fmax(m[5], fabs(ida * qa));
+    m[10] = fmax(m[10], fabs(qa + aty));
+    m[11] = fmax(m[11], fabs(aty));
+    m[12] = fmax(m[12], fabs(qa));
+  }
+}
+__device__ __forceinline__ void info_var_terms(const double dz, const double beta, const double x, const double zb,
+                                               const double aty, const double px, const double qv, double (&m)[14]) {
+  const double ax = beta * x;
+  const double einv = dz / beta, dinv = 1.0 / dz;
+  m[0] = fmax(m[0], fabs(einv * (ax - zb)));
+  m[1] = fmax(m[1], fabs(einv * zb));
+  m[2] = fmax(m[2], fabs(einv * ax));
+  m[7] = fmax(m[7], fabs(ax - zb));
+  m[8] = fmax(m[8], fabs(zb));
+  m[9] = fmax(m[9], fabs(ax));
+  const double d = qv + px + aty;
+  m[3] = fmax(m[3], fabs(dinv * d));
+  m[4] = fmax(m[4], fabs(dinv * aty));
+  m[5] = fmax(m[5], fabs(dinv * qv));
+  m[6] = fmax(m[6], fabs(dinv * px));
+  m[10] = fmax(m[10], fabs(d));
+  m[11] = fmax(m[11], fabs(aty));
+  m[12] = fmax(m[12], fabs(qv));
+  m[13] = fmax(m[13], fabs(px));
+}
+// first stage of the primal infeasibility certificate: a[0] |E dy| (max), a[1] u'dy+ + l'dy- (sum), a[2] |Dinv A_aux'dy|
+// (max).  Returns the projected dual step of the row (the column pass of the second stage scatters it).
+__device__ __forceinline__ double pinf_row_terms(const double* F, const int naux, double (&a)[3]) {
+  double d = F[R_DY];
+  d = (naux == AUX_HINGE) ? fmax(d, 0.0) : d;  // l = -inf
+  a[0] = fmax(a[0], fabs(F[R_E] * d));
+  a[1] += F[R_UP] * fmax(d, 0.0) + F[R_LO] * fmin(d, 0.0);
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    const double da = fmin(F[R_DYA0 + k], 0.0);  // aux bound rows: u = +inf, l = 0
+    a[0] = fmax(a[0], fabs(F[R_EA0 + k] * da));
+    a[2] = fmax(a[2], fabs((F[R_U0 + k] * d + F[R_B0 + k] * da) / F[R_DA0 + k]));
+  }
+  return d;
+}
+__device__ __forceinline__ void pinf_var_terms(const double ratio, const double ub, const double lb, const double d,
+                                               double (&a)[3]) {  // variable-bound rows: both bounds finite
+  a[0] = fmax(a[0], fabs(ratio * d));
+  a[1] += ub * fmax(d, 0.0) + lb * fmin(d, 0.0);
+}
+// first stage of the dual infeasibility certificate: a[0] |D dx| (max), a[1] q'dx (sum)
+__device__ __forceinline__ void dinf_row_terms(const double* F, double (&a)[2]) {
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    a[0] = fmax(a[0], fabs(F[R_DA0 + k] * F[R_DXA0 + k]));
+    a[1] += F[R_QA0 + k] * F[R_DXA0 + k];
+  }
+}
+// Hash of the active-set guess the polish would start from (optimisation O1): an order-independent sum (mod 2^64) of
+// one splitmix64 term per active row, keyed by the row's index in the canonical QP ([rows; trajectory bounds; aux
+// bounds]) and the side it is active on.
+__device__ __forceinline__ unsigned long long guess_mix(unsigned long long v) {
+  v += 0x9e3779b97f4a7c15ull;
+  v = (v ^ (v >> 30)) * 0xbf58476d1ce4e5b9ull;
+  v = (v ^ (v >> 27)) * 0x94d049bb133111ebull;
+  return v ^ (v >> 31);
+}
+__device__ __forceinline__ unsigned long long guess_row_hash(const double* F, const int* I, const int r, const int nrows,
+                                                             const int N) {
+  unsigned long long h = 0ull;
+  const unsigned long long mc = static_cast<unsigned long long>(nrows);
+  if (F[R_Z] - F[R_LO] < -F[R_Y]) h += guess_mix(2ull * r);
+  else if (F[R_UP] - F[R_Z] < F[R_Y]) h += guess_mix(2ull * r + 1ull);
+  for (int k = 0; k < I[RI_AUX]; ++k) {
+    const unsigned long long idx = mc + N + I[RI_PAD] + k;
+    if (F[R_ZA0 + k] - 0.0 < -F[R_YA0 + k]) h += guess_mix(2ull * idx);
+    else if (kOsqpInf * F[R_EA0 + k] - F[R_ZA0 + k] < F[R_YA0 + k]) h += guess_mix(2ull * idx + 1ull);
+  }
+  return h;
+}
+__device__ __forceinline__ unsigned long long guess_var_hash(const double zb, const double yb, const double lb,
+                                                             const double ub, const int i, const int nrows) {
+  const unsigned long long idx = static_cast<unsigned long long>(nrows) + i;
+  if (zb - lb < -yb) return guess_mix(2ull * idx);
+  if (ub - zb < yb) return guess_mix(2ull * idx + 1ull);
+  return 0ull;
+}
+// The check fused into admm_block_pinv leaves the warp partials of its quantities in the solver's Gauss-Jordan scratch
+// (q.tmp, unused between factorisations): quantity k of warp w at [k * 8 + w], the guess hash as a 64-bit word at
+// [kChkHash * 8 + w].  0..13 the norms of info_pass, then the first stages of the two certificates.
+enum ChkQ { CHK_PA0 = 14, CHK_PA1, CHK_PA2, CHK_DA0, CHK_DA1, kChkHash };
+constexpr unsigned kChkSumMask = (1u << CHK_PA1) | (1u << CHK_DA1);
 
 // per-row weights of the current linear system -> R_WRR (raw row weight), R_G0/G1, R_DEN, R_WR (Schur weight).
 // With the aux block K_aa = diag(g) + Wr u u' everything is written cancellation free (den = det K_aa
@@ -1790,6 +1908,9 @@ __device__ __noinline__ void admm_block_pinv(const QpCtx& q, const double rho_au
   constexpr int QN = 3 * NB;
   constexpr int kRowThreads = 64;  // warps 6-7
   extern __shared__ double sm[];
+#ifdef TB200_PROFILE
+  const long long prof_entry_ = clock64();
+#endif
   const int tid = q.tid, N = q.N, Np = q.Np, nrows = q.nrows, RS = q.RS;
   const double sigma = q.sigma, alpha = q.alpha, oma = 1.0 - q.alpha, rho = q.rho, rho_eq = q.rho_eq, rho_aux = rho_aux_in;
   const double inv_rho_aux = 1.0 / rho_aux, inv_rho = 1.0 / rho, inv_rho_eq = 1.0 / rho_eq;
@@ -1824,6 +1945,7 @@ __device__ __noinline__ void admm_block_pinv(const QpCtx& q, const double rho_au
   const bool v_eq = v_ub - v_lb < kRhoTol;
   const double v_rb = v_eq ? rho_eq : rho, v_irb = v_eq ? inv_rho_eq : inv_rho;
   double v_x = q.x[vi], v_z = q.zb[vi], v_y = q.yb[vi];
+  double v_dx = 0.0, v_dy = 0.0;  // the last iteration's steps (keep_last)
   const int e0 = has_var ? q.colptr[vi] : 0, e1 = has_var ? q.colptr[vi + 1] : 0;
   // a word that always reads 0.0 (the unused last scalar slot of the factorisation scratch)
   double* const zero_slot = sm + (q.flag - q.smbase) + 7;
@@ -1887,8 +2009,10 @@ __device__ __noinline__ void admm_block_pinv(const QpCtx& q, const double rho_au
       zn = fmin(fmax(zn, v_lb), v_ub);
       const double dy = v_rb * (zr - zn);
       if (keep_steps) {
-        dxs[vi] = xn - v_x;
-        dyb[vi] = dy;
+        v_dx = xn - v_x;
+        v_dy = dy;
+        dxs[vi] = v_dx;
+        dyb[vi] = v_dy;
       }
       v_x = xn;
       v_z = zn;
@@ -1902,6 +2026,9 @@ __device__ __noinline__ void admm_block_pinv(const QpCtx& q, const double rho_au
 #pragma unroll
     for (int j = 0; j < QN; ++j) pi[j] = prow ? q.pi_g[tid * QN + j] : 0.0;
     bar();  // (the entry pass of the row warps)
+#ifdef TB200_PROFILE
+    if (tid == 0) atomicAdd(&g_prof[21], (unsigned long long)(clock64() - prof_entry_));
+#endif
     for (int it = 0; it < n_iter; ++it) {
       const bool keep_steps = keep_last && it == n_iter - 1;
       { PROF_T0(); build_rhs(); PROF_ADD(1); }
@@ -2031,6 +2158,71 @@ __device__ __noinline__ void admm_block_pinv(const QpCtx& q, const double rho_au
     q.yb[vi] = v_y;
   }
   __syncthreads();
+  if (keep_last == 2) {
+    // ---- the terms of the termination check at the end of the block, in one pass (qp_solve_block reduces them where
+    // it needs them, fused_q) instead of the generic passes of info_pass, the certificates and the guess hash, with their ten-odd
+    // barriers.  Variables: their row of P x (p_matvec's order), A'y (scatter_columns' order), their norm terms, the
+    // certificates' first stages and the guess hash, from the state in registers; rows on warps 6-7.  The norms are
+    // maxima and the hash a wrapping sum, so they come out exactly as from the generic passes; the two floating-point
+    // sums of the certificates (u'dy+ + l'dy- and q'dx) are added in another order than there.
+    double m[14] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    double pa[3] = {0.0, 0.0, 0.0}, da[2] = {0.0, 0.0};
+    unsigned long long h = 0ull;
+    const double* const xs = sm + (q.x - q.smbase);
+    const double* const Dz = sm + (q.Dz - q.smbase);
+    if (has_var) {
+      const double px = p_row<NB>(q, vi, Dz, xs);
+      double aty = v_beta * v_y;
+      for (int e = e0; e < e1; ++e) {
+        const int ent = colent[e];
+        const double* R = rows + (ent >> 5) * RS;
+        aty += R[CNc + (ent & 31)] * R[2 * CNc + R_Y];
+      }
+      const double dz = Dz[vi];
+      info_var_terms(dz, v_beta, v_x, v_z, aty, px, v_qs, m);
+      pinf_var_terms(v_beta / dz, v_ub, v_lb, v_dy, pa);
+      da[0] = fmax(da[0], fabs(dz * v_dx));
+      da[1] += v_qs * v_dx;
+      h += guess_var_hash(v_z, v_y, v_lb, v_ub, vi, nrows);
+    }
+    if (upper) {
+      for (int r = kQpThreads - 1 - tid; r < nrows; r += kRowThreads) {
+        const double* R = rows + r * RS;
+        double* F = rows + r * RS + 2 * CNc;
+        const int* I = rints + r * RI_NINTS;
+        const double ax = row_dot<CNc>(q, R, I, xs) + F[R_U0] * F[R_XA0] + F[R_U1] * F[R_XA1];
+        info_row_terms(F, ax, m);
+        pinf_row_terms(F, I[RI_AUX], pa);
+        dinf_row_terms(F, da);
+        h += guess_row_hash(F, I, r, nrows, N);
+      }
+    }
+    // warp partials, reduced like block_reduce
+    double vals[kChkHash] = {m[0], m[1], m[2], m[3], m[4], m[5], m[6], m[7], m[8], m[9], m[10], m[11], m[12], m[13],
+                             pa[0], pa[1], pa[2], da[0], da[1]};
+    static_assert(CHK_PA0 == 14 && CHK_DA1 == 18, "vals[] follows ChkQ");
+    __syncwarp();
+#pragma unroll
+    for (int k = 0; k < kChkHash; ++k) {
+      double v = vals[k];
+      if ((kChkSumMask >> k) & 1u) {
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+      } else {
+        v = warp_max_norm(v);
+      }
+      vals[k] = v;
+    }
+    for (int off = 16; off > 0; off >>= 1) h += __shfl_xor_sync(0xffffffffu, h, off);
+    if ((tid & 31) == 0) {
+      double* const chk = sm + (q.tmp - q.smbase);
+      const int wid = tid >> 5;
+#pragma unroll
+      for (int k = 0; k < kChkHash; ++k) chk[k * 8 + wid] = vals[k];
+      reinterpret_cast<unsigned long long*>(chk + kChkHash * 8)[wid] = h;
+    }
+    __syncthreads();
+  }
 }
 
 // The block of iterations for QPs whose rows do not fit shared memory (configs[3] at 50 waypoints: ~370 rows of 14
@@ -2343,12 +2535,138 @@ __device__ inline void qp_scale(QpCtx& q, const QpSettings& st, int n_aux_total)
   __syncthreads();
 }
 
+// The refinement passes of the polish (qp_solve_block: polish_refine) for the partition-inverse layout: rows, row
+// index table, column entries, vectors and the cyclic-reduction factor of the polish system all in shared memory and
+// addressed as offsets, each variable's state in the registers of thread `i`, the rows on warps 6-7, and the solve
+// through fixed per-thread roles (bcr_solve_sm: the same products and sums as bcr_solve).  Its own function, called
+// through a pointer, for the reason of admm_block (§4.3 of DESIGN.md): inlined into qp_step, these passes ran on the
+// registers the solver's state leaves free and spilled.  Every value is the expression of polish_refine in its order,
+// so the polished point is bit for bit the same.  Needs Np <= kQpThreads and solve roles that fit the CTA.
+struct PolishRes {
+  double p_pri, p_dua, bad;  // max primal residual, max dual residual (scaled by c), wrongly signed multipliers
+};
+template <int NB, int PAIR>
+__device__ __noinline__ PolishRes polish_passes(const QpCtx& q, const int refine_iter) {
+  constexpr int CNc = PAIR ? ((NB > 3) ? NB : 3) : ((NB / 2 > 3) ? NB / 2 : 3);
+  constexpr int kRowThreads = 64;  // warps 6-7
+  extern __shared__ double sm[];
+  const int tid = q.tid, N = q.N, Np = q.Np, nrows = q.nrows, RS = q.RS;
+  double* const rows = sm + (q.rows - q.smbase);
+  const int* const rints = reinterpret_cast<const int*>(sm + (reinterpret_cast<const double*>(q.rints) - q.smbase));
+  const int* const colent = reinterpret_cast<const int*>(sm + (reinterpret_cast<const double*>(q.colent) - q.smbase));
+  double* const xs = sm + (q.x - q.smbase);
+  double* const v1 = sm + (q.v1 - q.smbase);
+  double* const w = sm + (q.w - q.smbase);
+  const double* const Dz = sm + (q.Dz - q.smbase);
+  const SolveRoles roles = solve_roles<NB>(q);
+  const bool upper = tid >= kQpThreads - kRowThreads;
+  // ---- this thread's variable (the polish weight's sign in zb: + upper bound active, - lower, 0 free)
+  const bool has_var = tid < N;
+  const int vi = has_var ? tid : 0;
+  const double v_beta = q.beta[vi], v_lb = q.lbs[vi], v_ub = q.ubs[vi], v_qs = q.qs[vi], v_dz = Dz[vi], v_zb = q.zb[vi];
+  const double v_w = fabs(v_zb), v_bnd = v_zb > 0 ? v_ub : v_lb;
+  const int e0 = has_var ? q.colptr[vi] : 0, e1 = has_var ? q.colptr[vi + 1] : 0;
+  double v_x = q.x[vi], v_y = q.yb[vi];
+  const double cinv = q.cinv;
+  __syncthreads();
+  for (int it = 0; it <= refine_iter + 1; ++it) {
+    const bool last = (it == refine_iter + 1);  // final pass: pending dual update + residuals only
+    double mm[3] = {0.0, 0.0, 0.0};             // m_pri (max), m_dua (max), bad signs (sum)
+    double px = 0.0;
+    if (has_var) px = p_row<NB>(q, vi, Dz, xs);  // (P xq)_i
+    if (upper) {
+      for (int r = kQpThreads - 1 - tid; r < nrows; r += kRowThreads) {
+        const double* R = rows + r * RS;
+        double* F = rows + r * RS + 2 * CNc;
+        const int* I = rints + r * RI_NINTS;
+        const int naux = I[RI_AUX];
+        const double Wr = F[R_WRR];
+        const double ax = row_dot<CNc>(q, R, I, xs) + F[R_U0] * F[R_PX0] + F[R_U1] * F[R_PX1];
+        const double py = F[R_PY] + ((it > 0) ? Wr * (ax - F[R_PB]) : 0.0);
+        const double e = py + (last ? 0.0 : Wr * (ax - F[R_PB]));
+        const double zc = fmin(fmax(ax, F[R_LO]), F[R_UP]);
+        mm[0] = fmax(mm[0], fabs((ax - zc) / F[R_E]));
+        mm[2] += (last && Wr != 0.0 && naux == AUX_HINGE && py < -kVerifyTol) ? 1.0 : 0.0;  // upper active needs y >= 0
+        double pya[2], ra[2];
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const double bb = F[R_B0 + k], u = F[R_U0 + k], qa = F[R_QA0 + k];
+          const double wa = fabs(F[R_PWA0 + k]);
+          const double axb = bb * F[R_PX0 + k];
+          pya[k] = F[R_PYA0 + k] + ((it > 0) ? wa * axb : 0.0);
+          const double ea = pya[k] + (last ? 0.0 : wa * axb);
+          mm[0] = fmax(mm[0], fabs((axb - fmax(axb, 0.0)) / F[R_EA0 + k]));
+          mm[2] += (last && wa != 0.0 && pya[k] > kVerifyTol) ? 1.0 : 0.0;  // aux >= 0 held at 0 needs y <= 0
+          mm[1] = fmax(mm[1], fabs((qa + u * py + bb * pya[k]) / F[R_DA0 + k]));
+          ra[k] = -qa - u * e - bb * ea;
+        }
+        F[R_PY] = py;
+        F[R_PYA0] = pya[0];
+        F[R_PYA1] = pya[1];
+        F[R_RA0] = ra[0];
+        F[R_RA1] = ra[1];
+        F[R_COEF] = last ? py : row_reduce_coef(F, ra[0], ra[1], -e);
+      }
+    }
+    __syncthreads();
+    // the variable's column: last pass the dual residual P x + q + A'y, else rd = -(P x + q) - beta (y + W (A x - b))
+    // + A' coef (scatter_columns' order)
+    if (tid < Np) {
+      double s = 0.0;
+      if (has_var) {
+        s = last ? px + v_qs + v_beta * v_y : -(px + v_qs) - v_beta * (v_y + v_w * (v_beta * v_x - v_bnd));
+        for (int e = e0; e < e1; ++e) {
+          const int ent = colent[e];
+          const double* R = rows + (ent >> 5) * RS;
+          s += R[CNc + (ent & 31)] * R[2 * CNc + R_COEF];
+        }
+        const double ax = v_beta * v_x;
+        const double zc = fmin(fmax(ax, v_lb), v_ub);
+        mm[0] = fmax(mm[0], fabs((ax - zc) * v_dz / v_beta));
+        const bool ineq = last && v_w != 0.0 && (v_ub - v_lb >= kRhoTol);
+        mm[2] += (ineq && v_zb > 0 && v_y < -kVerifyTol) ? 1.0 : 0.0;
+        mm[2] += (ineq && v_zb < 0 && v_y > kVerifyTol) ? 1.0 : 0.0;
+        if (last) mm[1] = fmax(mm[1], fabs(s / v_dz));
+      }
+      v1[tid] = s;
+    }
+    if (last) {
+      if (has_var) q.yb[vi] = v_y;
+      block_reduce<3, 0x4u>(q, mm);
+      return PolishRes{mm[0], mm[1] * cinv, mm[2]};
+    }
+    bcr_solve_sm<NB>(tid, roles, sm, v1, w);  // (begins with a barrier)
+    if (upper) {
+      for (int r = kQpThreads - 1 - tid; r < nrows; r += kRowThreads) {
+        const double* R = rows + r * RS;
+        double* F = rows + r * RS + 2 * CNc;
+        double a0, a1;
+        row_backsub(F, row_dot<CNc>(q, R, rints + r * RI_NINTS, w), a0, a1);
+        F[R_PX0] += a0;
+        F[R_PX1] += a1;
+      }
+    }
+    if (has_var) {
+      const double xn = v_x + w[vi];
+      // multiplier update of the variable-bound rows with the new iterate (the rows do theirs at the start of the
+      // next pass, where A x is recomputed anyway)
+      v_y += v_w * (v_beta * xn - v_bnd);
+      v_x = xn;
+      xs[vi] = xn;
+    }
+    __syncthreads();
+  }
+  return PolishRes{0.0, 0.0, 0.0};  // (not reached)
+}
+
 // The QP solve for the calling CTA's trajectory (initial iterate from the warm start or zero).
 // Every scalar that steers control flow is derived from block-reduced values, so all threads take the same path.
 // REGOK: the register-resident solve may be used (its per-thread factor rows fit the register file: blocks of <= 14).
+// fast_passes: the termination checks computed by the partition-inverse block (admm_block_pinv) and the polish
+// refinement by polish_passes, where the layout allows.
 template <int NB, int PAIR, bool REGOK>
 __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm, double warm_rho,
-                                       const double* ws_x, const double* ws_yb) {
+                                       const double* ws_x, const double* ws_yb, const bool fast_passes) {
   // coefficients per (padded) row: D, or 2*D when rows may span two consecutive waypoints (CartVel, cast collision)
   constexpr int CNc = PAIR ? ((NB > 3) ? NB : 3) : ((NB / 2 > 3) ? NB / 2 : 3);
   const int N = q.N, tid = q.tid;
@@ -2407,7 +2725,15 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
   // ... and short trajectories with their rows on chip use the partition-inverse form of the system (PinvPlan)
   const bool use_pinv = REGOK && q.pinv && q.rows_smem;
   using BlockFn = void (*)(const QpCtx&, double, int, int);
+  // fast_passes: the partition-inverse block can end in the terms of a termination check, and the polish refinement
+  // runs as polish_passes (else the generic passes of this function)
+  const bool fuse = use_pinv && fast_passes;
+  const bool fast_polish = use_pinv && fast_passes && q.Np <= kQpThreads && solve_roles_fit(q.M, NB);
+  // q.tmp holds the fused check's partials of the current iterate: set by a block that computed them, cleared by every
+  // factorisation (it reuses q.tmp)
+  bool fused_chk = false;
   auto run_block = [&](int n, bool keep_last) {
+    fused_chk = fuse && keep_last;
     if constexpr (REGOK) {
       if (use_pinv || use_reg) {
         // (called through pointers: an indirect call follows the standard calling convention, so the block gets the
@@ -2416,7 +2742,7 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
         // the loop and every level of its solve is scheduled one shared-memory load at a time.)
         BlockFn volatile fn = use_pinv ? &admm_block_pinv<NB, PAIR>
                                        : (q.rows_smem ? &admm_block_fast<NB, PAIR> : &admm_block_soa<NB, PAIR>);
-        fn(q, sysw.rho_aux, n, keep_last ? 1 : 0);
+        fn(q, sysw.rho_aux, n, keep_last ? (fuse ? 2 : 1) : 0);
         return;
       }
     }
@@ -2428,6 +2754,7 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
   // takes the cyclic reduction (its solves are the generic ones)
   using FactorFn = bool (*)(const QpCtx&, const SysW&);
   auto factorize = [&](const SysW& wts) -> bool {
+    fused_chk = false;
     if constexpr (REGOK) {
       if (use_pinv && !wts.polish) {
         FactorFn volatile fn = &assemble_factor<NB, true>;
@@ -2477,59 +2804,14 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
       const double* R = q.R(r);
       double* F = q.F(r);
       const double ax = row_dot<CNc>(q, R, q.I(r), q.x) + F[R_U0] * F[R_XA0] + F[R_U1] * F[R_XA1];
-      const double einv = 1.0 / F[R_E];
-      m[0] = fmax(m[0], fabs(einv * (ax - F[R_Z])));
-      m[1] = fmax(m[1], fabs(einv * F[R_Z]));
-      m[2] = fmax(m[2], fabs(einv * ax));
-      m[7] = fmax(m[7], fabs(ax - F[R_Z]));
-      m[8] = fmax(m[8], fabs(F[R_Z]));
-      m[9] = fmax(m[9], fabs(ax));
-#pragma unroll
-      for (int k = 0; k < 2; ++k) {  // absent aux slots contribute exact zeros
-        const double u = F[R_U0 + k], bb = F[R_B0 + k], qa = F[R_QA0 + k];
-        const double xa = F[R_XA0 + k], za = F[R_ZA0 + k], ya = F[R_YA0 + k];
-        // Einv / Dinv of the aux row and column: one reciprocal each, multiplied like the Einv[r] * (...) of the oracle
-        const double iea = 1.0 / F[R_EA0 + k], ida = 1.0 / F[R_DA0 + k];
-        const double axb = bb * xa;
-        m[0] = fmax(m[0], fabs(iea * (axb - za)));
-        m[1] = fmax(m[1], fabs(iea * za));
-        m[2] = fmax(m[2], fabs(iea * axb));
-        m[7] = fmax(m[7], fabs(axb - za));
-        m[8] = fmax(m[8], fabs(za));
-        m[9] = fmax(m[9], fabs(axb));
-        const double aty = u * F[R_Y] + bb * ya;
-        m[3] = fmax(m[3], fabs(ida * (qa + aty)));
-        m[4] = fmax(m[4], fabs(ida * aty));
-        m[5] = fmax(m[5], fabs(ida * qa));
-        m[10] = fmax(m[10], fabs(qa + aty));
-        m[11] = fmax(m[11], fabs(aty));
-        m[12] = fmax(m[12], fabs(qa));
-      }
+      info_row_terms(F, ax, m);
       F[R_COEF] = F[R_Y];
     }
     __syncthreads();
     PROF_CHK(14);
     scatter_columns<CNc>(q, [&](int i) { return q.beta[i] * q.yb[i]; });  // v1 <- A'y (trajectory part)
-    for (int i = tid; i < N; i += kQpThreads) {
-      const double dz = q.Dz[i], beta = q.beta[i];
-      const double ax = beta * q.x[i], aty = q.v1[i], px = q.v2[i];
-      const double einv = dz / beta, dinv = 1.0 / dz;
-      m[0] = fmax(m[0], fabs(einv * (ax - q.zb[i])));
-      m[1] = fmax(m[1], fabs(einv * q.zb[i]));
-      m[2] = fmax(m[2], fabs(einv * ax));
-      m[7] = fmax(m[7], fabs(ax - q.zb[i]));
-      m[8] = fmax(m[8], fabs(q.zb[i]));
-      m[9] = fmax(m[9], fabs(ax));
-      const double qv = q.qs[i], d = qv + px + aty;
-      m[3] = fmax(m[3], fabs(dinv * d));
-      m[4] = fmax(m[4], fabs(dinv * aty));
-      m[5] = fmax(m[5], fabs(dinv * qv));
-      m[6] = fmax(m[6], fabs(dinv * px));
-      m[10] = fmax(m[10], fabs(d));
-      m[11] = fmax(m[11], fabs(aty));
-      m[12] = fmax(m[12], fabs(qv));
-      m[13] = fmax(m[13], fabs(px));
-    }
+    for (int i = tid; i < N; i += kQpThreads)
+      info_var_terms(q.Dz[i], q.beta[i], q.x[i], q.zb[i], q.v1[i], q.v2[i], q.qs[i], m);
     if (scaled) {  // (block-uniform)
       block_reduce<14, 0u>(q, m);
       s_pri = m[7]; s_z = m[8]; s_ax = m[9]; s_dua = m[10]; s_aty = m[11]; s_q = m[12]; s_px = m[13];
@@ -2545,30 +2827,55 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
     n_z = m[1]; n_ax = m[2]; n_aty = m[4]; n_q = m[5]; n_px = m[6];
   };
 
+  // The check fused into the last iteration of an ADMM block (admm_block_pinv, keep_last == 2): quantity k (ChkQ)
+  // reduced from its warp partials in q.tmp, in the order of block_reduce.  Read where each quantity is needed (nothing
+  // of it is carried across the ADMM loop); every writer of q.tmp is behind a barrier that follows these reads.
+  auto fused_q = [&](const int k) -> double {
+    extern __shared__ double sm[];
+    const double* const chk = sm + (q.tmp - q.smbase) + k * 8;
+    if ((kChkSumMask >> k) & 1u) {
+      double acc = chk[0];
+      for (int w = 1; w < kQpThreads / 32; ++w) acc += chk[w];
+      return acc;
+    }
+    return warp_max_norm(chk[tid & 7]);
+  };
+  // the residuals of the current iterate: from the fused check when q.tmp holds it
+  auto residuals = [&](const bool scaled) {
+    if (!fused_chk) {
+      info_pass(scaled);
+      return;
+    }
+    double m[14];
+#pragma unroll
+    for (int k = 0; k < 14; ++k) m[k] = (k < 7 || scaled) ? fused_q(k) : 0.0;
+    pri_res = m[0];
+    dua_res = m[3] * q.cinv;
+    n_z = m[1]; n_ax = m[2]; n_aty = m[4]; n_q = m[5]; n_px = m[6];
+    if (scaled) { s_pri = m[7]; s_z = m[8]; s_ax = m[9]; s_dua = m[10]; s_aty = m[11]; s_q = m[12]; s_px = m[13]; }
+  };
+
   auto primal_infeasible = [&](double eps) -> bool {  // is_primal_infeasible [EXT]
     double a[3] = {0.0, 0.0, 0.0};  // nd (max), lhs (sum), na (max)
-    for (int r = tid; r < q.nrows; r += kQpThreads) {
-      double* F = q.F(r);
-      const int naux = q.I(r)[RI_AUX];
-      double d = F[R_DY];
-      d = (naux == AUX_HINGE) ? fmax(d, 0.0) : d;  // l = -inf
-      a[0] = fmax(a[0], fabs(F[R_E] * d));
-      a[1] += F[R_UP] * fmax(d, 0.0) + F[R_LO] * fmin(d, 0.0);
-      F[R_COEF] = d;  // projected dual step, consumed by the column pass
-#pragma unroll
-      for (int k = 0; k < 2; ++k) {
-        const double da = fmin(F[R_DYA0 + k], 0.0);  // aux bound rows: u = +inf, l = 0
-        a[0] = fmax(a[0], fabs(F[R_EA0 + k] * da));
-        a[2] = fmax(a[2], fabs((F[R_U0 + k] * d + F[R_B0 + k] * da) / F[R_DA0 + k]));
+    if (fused_chk) {
+      a[0] = fused_q(CHK_PA0); a[1] = fused_q(CHK_PA1); a[2] = fused_q(CHK_PA2);
+    } else {
+      for (int r = tid; r < q.nrows; r += kQpThreads) {
+        double* F = q.F(r);
+        F[R_COEF] = pinf_row_terms(F, q.I(r)[RI_AUX], a);  // projected dual step, consumed by the column pass
       }
+      for (int i = tid; i < N; i += kQpThreads) pinf_var_terms(q.beta[i] / q.Dz[i], q.ubs[i], q.lbs[i], dyb[i], a);
+      block_reduce<3, 0x2u>(q, a);
     }
-    for (int i = tid; i < N; i += kQpThreads) {  // variable-bound rows: both bounds finite
-      const double d = dyb[i];
-      a[0] = fmax(a[0], fabs(q.beta[i] / q.Dz[i] * d));
-      a[1] += q.ubs[i] * fmax(d, 0.0) + q.lbs[i] * fmin(d, 0.0);
-    }
-    block_reduce<3, 0x2u>(q, a);
     if (!((a[0] > eps) && (a[1] < -eps * a[0]))) return false;  // block-uniform: the A'dy test cannot rescue it
+    if (fused_chk) {  // the projected dual steps for the column pass (the generic first stage leaves them in R_COEF)
+      double unused[3] = {0.0, 0.0, 0.0};
+      for (int r = tid; r < q.nrows; r += kQpThreads) {
+        double* F = q.F(r);
+        F[R_COEF] = pinf_row_terms(F, q.I(r)[RI_AUX], unused);
+      }
+      __syncthreads();
+    }
     scatter_columns<CNc>(q, [&](int i) { return q.beta[i] * dyb[i]; });
     double mm[1] = {a[2]};
     for (int i = tid; i < N; i += kQpThreads) mm[0] = fmax(mm[0], fabs(q.v1[i] / q.Dz[i]));
@@ -2577,25 +2884,20 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
   };
   auto dual_infeasible = [&](double eps) -> bool {  // is_dual_infeasible [EXT]
     double a[2] = {0.0, 0.0};  // ndx (max), qdx (sum)
-    for (int i = tid; i < q.Np; i += kQpThreads) {
-      const double dxi = (i < N) ? dxs[i] : 0.0;
-      if (i < N) {
-        a[0] = fmax(a[0], fabs(q.Dz[i] * dxi));
-        a[1] += q.qs[i] * dxi;
+    if (fused_chk) {
+      a[0] = fused_q(CHK_DA0); a[1] = fused_q(CHK_DA1);
+    } else {
+      for (int i = tid; i < N; i += kQpThreads) {
+        a[0] = fmax(a[0], fabs(q.Dz[i] * dxs[i]));
+        a[1] += q.qs[i] * dxs[i];
       }
-      q.v1[i] = dxi;
+      for (int r = tid; r < q.nrows; r += kQpThreads) dinf_row_terms(q.F(r), a);
+      block_reduce<2, 0x2u>(q, a);
     }
-    for (int r = tid; r < q.nrows; r += kQpThreads) {
-      const double* F = q.F(r);
-#pragma unroll
-      for (int k = 0; k < 2; ++k) {
-        a[0] = fmax(a[0], fabs(F[R_DA0 + k] * F[R_DXA0 + k]));
-        a[1] += F[R_QA0 + k] * F[R_DXA0 + k];
-      }
-    }
-    block_reduce<2, 0x2u>(q, a);
     const double ndx = a[0], qdx = a[1];
     if (!((ndx > eps) && (qdx < -q.c * eps * ndx))) return false;  // block-uniform: skip the P dx / A dx tests
+    for (int i = tid; i < q.Np; i += kQpThreads) q.v1[i] = (i < N) ? dxs[i] : 0.0;
+    __syncthreads();
     p_matvec<NB>(q, q.v1, q.v2);  // v2 <- P dx
     double b2[2] = {0.0, 0.0};  // max |Dinv P dx|, bad count (sum)
     for (int i = tid; i < N; i += kQpThreads) {
@@ -2641,44 +2943,27 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
   };
 
   // ---------------------------------------------------------------- optimisation O1: when to try the polish early
-  // Hash of the active-set guess the polish would start from: an order-independent sum (mod 2^64) of one
-  // splitmix64 term per active row, keyed by the row's index in the canonical QP ([rows; trajectory bounds;
-  // aux bounds]) and the side it is active on.  The polish is tried early only when the guess is the same as at
-  // the previous test and has not failed before.
-  auto guess_mix = [](unsigned long long v) -> unsigned long long {
-    v += 0x9e3779b97f4a7c15ull;
-    v = (v ^ (v >> 30)) * 0xbf58476d1ce4e5b9ull;
-    v = (v ^ (v >> 27)) * 0x94d049bb133111ebull;
-    return v ^ (v >> 31);
-  };
+  // The polish is tried early only when the hash of the active-set guess (guess_row_hash / guess_var_hash) is the same
+  // as at the previous test and has not failed before.
   auto early_guess_settled = [&]() -> bool {
     unsigned long long h = 0ull;
-    const unsigned long long mc = static_cast<unsigned long long>(q.nrows);
-    for (int r = tid; r < q.nrows; r += kQpThreads) {
-      const double* F = q.F(r);
-      const int* I = q.I(r);
-      if (F[R_Z] - F[R_LO] < -F[R_Y]) h += guess_mix(2ull * r);
-      else if (F[R_UP] - F[R_Z] < F[R_Y]) h += guess_mix(2ull * r + 1ull);
-      for (int k = 0; k < I[RI_AUX]; ++k) {
-        const unsigned long long idx = mc + N + I[RI_PAD] + k;
-        if (F[R_ZA0 + k] - 0.0 < -F[R_YA0 + k]) h += guess_mix(2ull * idx);
-        else if (kOsqpInf * F[R_EA0 + k] - F[R_ZA0 + k] < F[R_YA0 + k]) h += guess_mix(2ull * idx + 1ull);
-      }
+    if (fused_chk) {
+      extern __shared__ double sm[];
+      const unsigned long long* hw = reinterpret_cast<const unsigned long long*>(sm + (q.tmp - q.smbase) + kChkHash * 8);
+      for (int w = 0; w < kQpThreads / 32; ++w) h += hw[w];
+    } else {
+      for (int r = tid; r < q.nrows; r += kQpThreads) h += guess_row_hash(q.F(r), q.I(r), r, q.nrows, N);
+      for (int i = tid; i < N; i += kQpThreads) h += guess_var_hash(q.zb[i], q.yb[i], q.lbs[i], q.ubs[i], i, q.nrows);
+      // block sum (wraps): butterfly inside the warp, then the 8 partials through shared memory
+      __syncwarp();
+      for (int off = 16; off > 0; off >>= 1) h += __shfl_xor_sync(0xffffffffu, h, off);
+      unsigned long long* red = reinterpret_cast<unsigned long long*>(q.red.ptr());
+      if ((tid & 31) == 0) red[tid >> 5] = h;
+      __syncthreads();
+      h = 0ull;
+      for (int w = 0; w < kQpThreads / 32; ++w) h += red[w];
+      __syncthreads();
     }
-    for (int i = tid; i < N; i += kQpThreads) {
-      const unsigned long long idx = mc + i;
-      if (q.zb[i] - q.lbs[i] < -q.yb[i]) h += guess_mix(2ull * idx);
-      else if (q.ubs[i] - q.zb[i] < q.yb[i]) h += guess_mix(2ull * idx + 1ull);
-    }
-    // block sum (wraps): butterfly inside the warp, then the 8 partials through shared memory
-    __syncwarp();
-    for (int off = 16; off > 0; off >>= 1) h += __shfl_xor_sync(0xffffffffu, h, off);
-    unsigned long long* red = reinterpret_cast<unsigned long long*>(q.red.ptr());
-    if ((tid & 31) == 0) red[tid >> 5] = h;
-    __syncthreads();
-    h = 0ull;
-    for (int w = 0; w < kQpThreads / 32; ++w) h += red[w];
-    __syncthreads();
     const bool stable = have_prev_guess && h == prev_guess;
     prev_guess = h;
     have_prev_guess = true;
@@ -2692,7 +2977,7 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
     bool stop = false;
     while (!stop) {
       if (iter >= st.max_iter) {  // max_iter reached without a verdict: approximate test, then MAX_ITER_REACHED
-        if (!(st.check_termination > 0 && (iter % st.check_termination == 0))) info_pass(false);
+        if (!(st.check_termination > 0 && (iter % st.check_termination == 0))) residuals(false);
         status = check_termination(true);
         if (status == QPS_UNSOLVED) status = QPS_MAXITER;
         stop = true;
@@ -2707,19 +2992,26 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
         run_block(n, can_check || iter == st.max_iter);
         if (can_check) {
           PROF_T0();
-          info_pass(rho_iter);
+          residuals(rho_iter);
           PROF_CHK_T0();
           status = check_termination(false);
           PROF_CHK(9);
           PROF_ADD(5);
+          bool try_early = false;
           if (status != QPS_UNSOLVED) stop = true;
           else if (st.polishing && st.early_polish_every > 0 && iter >= st.early_polish_from &&
-                   (iter % st.early_polish_every == 0) && early_guess_settled()) {
+                   (iter % st.early_polish_every == 0)) {
+            PROF_T0();
+            try_early = early_guess_settled();
+            PROF_ADD(22);
+          }
+          if (try_early) {
             // optimisation O1: try the polish before ADMM has met its own tolerances; a VERIFIED polished point
             // is the exact minimiser no matter how rough the iterate that produced the active-set guess was
             bool verified = false;
             double p_pri = 0.0, p_dua = 0.0;
-            if (use_pinv) stash_z(false);
+            PROF_COUNT(17);
+            { PROF_T0(); if (use_pinv) stash_z(false); PROF_ADD(16); }
             const bool factored = polish_fn(verified, p_pri, p_dua);
             if (factored && verified) {
               early_verified = true;
@@ -2729,21 +3021,26 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
               status = QPS_SOLVED;
               stop = true;
             } else {
+              PROF_T0();
               failed_guess = pending_guess;
               have_failed_guess = true;
+              // x, zb, yb come back exactly and the polish writes none of the row fields the residual norms read, so
+              // the residual scalars of this check (pri_res, dua_res, n_*, s_*) still hold: no second info_pass.  (It
+              // does overwrite R_COEF and, through its factorisation, q.tmp: a certificate evaluated after this point
+              // takes the generic first stage, which rebuilds both from the iterate.)
               restore_fn(false);
-              info_pass(rho_iter);  // the polish reuses the vectors of the residual bookkeeping
               if (use_pinv) {
                 stash_z(true);
               } else if (!factorize(sysw)) {
                 status = QPS_NONCVX;
                 stop = true;
               }
+              PROF_ADD(19);
             }
           }
         }
         if (!stop && rho_iter) {
-          if (!can_check) info_pass(true);
+          if (!can_check) residuals(true);
           // compute_rho_estimate on the scaled quantities [EXT]
           const double pn = s_pri / (fmax(s_z, s_ax) + 1e-10);
           const double dn = s_dua / (fmax(s_q, fmax(s_aty, s_px)) + 1e-10);
@@ -2755,10 +3052,12 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
             q.rho_eq = kRhoEqOverIneq * rho;
             sysw.rho_aux = rho;
             out.rho_updates++;
+            PROF_T0();
             if (!factorize(sysw)) {
               status = QPS_NONCVX;
               stop = true;
             }
+            PROF_ADD(20);
           }
         }
       }
@@ -2773,46 +3072,21 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
   // correctly signed multiplier, i.e. it is a KKT point of the QP = the unique minimiser.
   const double wp = 1.0 / st.delta;
   const SysW pw{true, st.delta, 0.0};
-  auto polish_once = [&](bool& verified, double& p_pri, double& p_dua) -> bool {
+  // the refinement passes on the factored polish system
+  auto polish_refine = [&](bool& verified, double& p_pri, double& p_dua) {
     PROF_T0();
-    verified = false;
-    for (int i = tid; i < q.Np; i += kQpThreads) {
-      const double z = q.zb[i], y = q.yb[i];
-      double w = 0.0;
-      if (i < N) {
-        if (z - q.lbs[i] < -y) w = -wp;           // lower active
-        else if (q.ubs[i] - z < y) w = wp;        // upper active
-      }
-      st_x[i] = q.x[i];
-      st_zb[i] = z;
-      st_yb[i] = y;
-      q.zb[i] = w;                                 // signed polish weight
-      q.x[i] = 0.0;                                // polish iterate
-      q.yb[i] = 0.0;                               // polish multiplier
-    }
-    for (int r = tid; r < q.nrows; r += kQpThreads) {
-      double* F = q.F(r);
-      const int naux = q.I(r)[RI_AUX];
-      double w = 0.0, b = 0.0;
-      if (F[R_Z] - F[R_LO] < -F[R_Y]) { w = -wp; b = F[R_LO]; }
-      else if (F[R_UP] - F[R_Z] < F[R_Y]) { w = wp; b = F[R_UP]; }
-      F[R_PW] = w;
-      F[R_PB] = b;
-      F[R_PY] = 0.0;
-#pragma unroll
-      for (int k = 0; k < 2; ++k) {
-        double wa = 0.0;
-        if (k < naux) {
-          if (F[R_ZA0 + k] - 0.0 < -F[R_YA0 + k]) wa = -wp;                                    // lower (0) active
-          else if (kOsqpInf * F[R_EA0 + k] - F[R_ZA0 + k] < F[R_YA0 + k]) wa = wp;            // never in practice
-        }
-        F[R_PWA0 + k] = wa;
-        F[R_PYA0 + k] = 0.0;
-        F[R_PX0 + k] = 0.0;
+    if constexpr (REGOK) {
+      if (fast_polish) {
+        using PassFn = PolishRes (*)(const QpCtx&, int);
+        PassFn volatile fn = &polish_passes<NB, PAIR>;
+        const PolishRes res = fn(q, st.polish_refine_iter);
+        p_pri = res.p_pri;
+        p_dua = res.p_dua;
+        verified = (res.bad == 0.0) && (p_pri <= kVerifyTol) && isfinite(p_pri) && isfinite(p_dua);
+        PROF_ADD(12);
+        return;
       }
     }
-    __syncthreads();
-    if (!factorize(pw)) return false;
     for (int it = 0; it <= st.polish_refine_iter + 1; ++it) {
       const bool last = (it == st.polish_refine_iter + 1);  // final pass: pending dual update + residuals only
       p_matvec<NB>(q, q.x, q.v2);  // v2 <- P xq
@@ -2901,9 +3175,52 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
       }
     }
     PROF_ADD(12);
-#ifdef TB200_PROFILE
-    if (tid == 0) atomicAdd(&g_prof[13], 1ull);
-#endif
+  };
+  auto polish_once = [&](bool& verified, double& p_pri, double& p_dua) -> bool {
+    PROF_COUNT(13);
+    PROF_T0();
+    verified = false;
+    for (int i = tid; i < q.Np; i += kQpThreads) {
+      const double z = q.zb[i], y = q.yb[i];
+      double w = 0.0;
+      if (i < N) {
+        if (z - q.lbs[i] < -y) w = -wp;           // lower active
+        else if (q.ubs[i] - z < y) w = wp;        // upper active
+      }
+      st_x[i] = q.x[i];
+      st_zb[i] = z;
+      st_yb[i] = y;
+      q.zb[i] = w;                                 // signed polish weight
+      q.x[i] = 0.0;                                // polish iterate
+      q.yb[i] = 0.0;                               // polish multiplier
+    }
+    for (int r = tid; r < q.nrows; r += kQpThreads) {
+      double* F = q.F(r);
+      const int naux = q.I(r)[RI_AUX];
+      double w = 0.0, b = 0.0;
+      if (F[R_Z] - F[R_LO] < -F[R_Y]) { w = -wp; b = F[R_LO]; }
+      else if (F[R_UP] - F[R_Z] < F[R_Y]) { w = wp; b = F[R_UP]; }
+      F[R_PW] = w;
+      F[R_PB] = b;
+      F[R_PY] = 0.0;
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        double wa = 0.0;
+        if (k < naux) {
+          if (F[R_ZA0 + k] - 0.0 < -F[R_YA0 + k]) wa = -wp;                                    // lower (0) active
+          else if (kOsqpInf * F[R_EA0 + k] - F[R_ZA0 + k] < F[R_YA0 + k]) wa = wp;            // never in practice
+        }
+        F[R_PWA0 + k] = wa;
+        F[R_PYA0 + k] = 0.0;
+        F[R_PX0 + k] = 0.0;
+      }
+    }
+    __syncthreads();
+    PROF_ADD(16);
+    bool factored;
+    { PROF_T0(); factored = factorize(pw); PROF_ADD(23); }
+    if (!factored) return false;
+    polish_refine(verified, p_pri, p_dua);
     return true;
   };
   auto restore_admm_state = [&](bool keep_polished_x) {
@@ -2931,7 +3248,8 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
     } else {
       bool verified = false;
       double p_pri = 0.0, p_dua = 0.0;
-      if (use_pinv) stash_z(false);
+      PROF_COUNT(18);
+      { PROF_T0(); if (use_pinv) stash_z(false); PROF_ADD(16); }
       const bool factored = polish_once(verified, p_pri, p_dua);
       out.pol_factor_ok = factored ? 1 : 0;
       out.pol_pri = p_pri;
@@ -2948,6 +3266,7 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
       } else {
         ++round;
         eps_scale *= 0.1;
+        PROF_T0();
         restore_admm_state(false);
         if (use_pinv) {  // back to the ADMM factor
           stash_z(true);
@@ -2955,6 +3274,7 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
           status = QPS_NONCVX;
           done = true;
         }
+        PROF_ADD(19);
       }
     }
   }
@@ -3274,7 +3594,7 @@ __device__ __noinline__ void qp_step(const DevProblem& p, const int b, const dou
 
   PROF_T0();
   QpOut res = qp_solve_block<NB, PAIR, (DD <= 7)>(q, p.qp, warm, p.ws_rho[b], p.ws_x + static_cast<size_t>(b) * N,
-                                                  p.ws_yb + static_cast<size_t>(b) * N);
+                                                  p.ws_yb + static_cast<size_t>(b) * N, p.qp_fast_passes != 0);
   __syncthreads();
   PROF_ADD(8);
 #ifdef TB200_PROFILE

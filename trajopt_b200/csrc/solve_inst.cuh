@@ -16,14 +16,15 @@ SolveKernelFn TB200_CAT3(solve_kernel_inst_, TB200_INST_D, TB200_INST_PAIR)() {
 // TB200_PROFILE builds: the phase counters of this translation unit (else -1)
 int TB200_CAT3(qp_prof_inst_, TB200_INST_D, TB200_INST_PAIR)(unsigned long long* out, int reset) {
 #ifdef TB200_PROFILE
+  static_assert(sizeof(g_prof) == kQpProfSlots * sizeof(unsigned long long), "g_prof and kQpProfSlots disagree");
   if (reset) {
-    unsigned long long z[16] = {0};
+    unsigned long long z[kQpProfSlots] = {0};
     cudaMemcpyToSymbol(g_prof, z, sizeof(z));
     return 0;
   }
-  unsigned long long t[16];
+  unsigned long long t[kQpProfSlots];
   cudaMemcpyFromSymbol(t, g_prof, sizeof(t));
-  for (int i = 0; i < 16; ++i) out[i] += t[i];
+  for (int i = 0; i < kQpProfSlots; ++i) out[i] += t[i];
   return 0;
 #else
   (void)out;

@@ -21,7 +21,7 @@ SolveKernelFn solve_kernel_for(int D, bool pair_rows) {
 int qp_debug_prof(unsigned long long* out, int reset) {
   int rc = -1;
   if (!reset && out)
-    for (int i = 0; i < 16; ++i) out[i] = 0;
+    for (int i = 0; i < kQpProfSlots; ++i) out[i] = 0;
 #define TB200_PROF(D, P) \
   if (qp_prof_inst_##D##_##P(out, reset) == 0) rc = 0;
   TB200_INSTANCES(TB200_PROF)

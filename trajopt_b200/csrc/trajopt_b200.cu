@@ -545,6 +545,12 @@ int tb200_problem_create(const tb200_problem_desc* d, int device, tb200_problem*
     P->n_sm = std::max(1, sms);
   }
   if (const char* e = std::getenv("TB200_QUANTUM")) P->quantum = std::max(1, std::atoi(e));
+  // TB200_GENERIC_QP_PASSES=1: termination checks and polish refinement by the generic passes of the QP solver instead
+  // of the check fused into the ADMM block and polish_passes (same decisions; the switch exists to compare the two)
+  {
+    const char* e = std::getenv("TB200_GENERIC_QP_PASSES");
+    P->dp.qp_fast_passes = (e && std::atoi(e) != 0) ? 0 : 1;
+  }
   CK(cudaStreamCreateWithFlags(&P->stream, cudaStreamNonBlocking));
 
   // ---- device buffers ------------------------------------------------------------------------------------
