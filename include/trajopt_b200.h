@@ -30,7 +30,7 @@ extern "C" {
 #endif
 
 #define TB200_VERSION_MAJOR 0
-#define TB200_VERSION_MINOR 1
+#define TB200_VERSION_MINOR 2
 #define TB200_MAX_DOF 16      /* joints per manipulator group (7 single arm, 14 dual arm) */
 #define TB200_MAX_STEPS 64    /* waypoints per trajectory */
 #define TB200_MIN_CAST_ROWS_PER_PAIR 128  /* continuous collision evaluators: lower / upper limit of the active contacts */
@@ -155,6 +155,10 @@ typedef struct tb200_sqp_params {
   double trust_box_size;
   int32_t inflate_constraints_individually;
   int32_t reserved;
+  /* wall-clock budget of a solve in seconds (optimizers.cpp:738-753); DBL_MAX = none.  Checked at the top of every SQP
+   * iteration: a trajectory past it ends with its last accepted iterate, OPT_CONVERGED when its constraints are within
+   * cnt_tolerance (or it has none), else OPT_TIME_LIMIT.  One device clock per solve (DESIGN.md section 6). */
+  double max_time;
 } tb200_sqp_params;
 
 /* OSQPSettings as set by OSQPModelConfig::setDefaultOSQPSettings (osqp_interface.cpp:78-90)

@@ -60,6 +60,7 @@ struct BasicTrustRegionSQPParameters {
   double initial_merit_error_coeff = 10;
   bool inflate_constraints_individually = true;
   double trust_box_size = 1e-1;
+  double max_time = std::numeric_limits<double>::max();  // seconds (DESIGN.md section 6: one device clock per batch)
 };
 
 // optimizers.hpp:40-59
@@ -423,6 +424,8 @@ inline std::shared_ptr<FlatProblem> FlattenProblem(const ProblemConstructionInfo
   d.sqp.initial_merit_error_coeff = p.initial_merit_error_coeff;
   d.sqp.trust_box_size = p.trust_box_size;
   d.sqp.inflate_constraints_individually = p.inflate_constraints_individually ? 1 : 0;
+  d.sqp.reserved = 0;
+  d.sqp.max_time = p.max_time;
   return fp;
 }
 

@@ -320,6 +320,7 @@ inline void fromJson(ProblemConstructionInfo& pci, const json::Value& v, const s
     json_marshal::childFromJson(o, p.cnt_tolerance, "cnt_tolerance", d.cnt_tolerance);
     json_marshal::childFromJson(o, p.max_merit_coeff_increases, "max_merit_coeff_increases", d.max_merit_coeff_increases);
     json_marshal::childFromJson(o, p.merit_coeff_increase_ratio, "merit_coeff_increase_ratio", d.merit_coeff_increase_ratio);
+    json_marshal::childFromJson(o, p.max_time, "max_time", d.max_time);
     json_marshal::childFromJson(o, p.initial_merit_error_coeff, "initial_merit_error_coeff", d.initial_merit_error_coeff);
     json_marshal::childFromJson(o, p.inflate_constraints_individually, "inflate_constraints_individually", d.inflate_constraints_individually);
     json_marshal::childFromJson(o, p.trust_box_size, "trust_box_size", d.trust_box_size);

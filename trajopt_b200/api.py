@@ -53,6 +53,10 @@ class Problem:
         keep = [np.ascontiguousarray(a, dtype=np.float64) if a is not None else None for a in (init_traj, cart_targets, obstacles)]
         self._check(self.lib.tb200_problem_set_inputs(self.handle, *[None if a is None else _dp(a) for a in keep]))
 
+    def set_sqp_params(self, sqp):
+        """Replace the optimizer parameters (a capi.SqpParams, e.g. with a new max_time) for the next solves."""
+        self._check(self.lib.tb200_problem_set_sqp_params(self.handle, C.byref(sqp)))
+
     def _results(self):
         L, d = self.layout, self.desc
         return capi.alloc_results(d.B, d.T, d.D, L.n_costs, L.n_cnts)

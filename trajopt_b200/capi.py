@@ -60,7 +60,7 @@ class SqpParams(C.Structure):
                 ("cnt_tolerance", C.c_double), ("max_merit_coeff_increases", C.c_double),
                 ("merit_coeff_increase_ratio", C.c_double), ("initial_merit_error_coeff", C.c_double),
                 ("trust_box_size", C.c_double), ("inflate_constraints_individually", C.c_int32),
-                ("reserved", C.c_int32)]
+                ("reserved", C.c_int32), ("max_time", C.c_double)]
 
 
 class QpSettings(C.Structure):
@@ -126,6 +126,7 @@ def default_sqp_params():
     p.initial_merit_error_coeff = 10
     p.trust_box_size = 0.1
     p.inflate_constraints_individually = 1
+    p.max_time = np.finfo(np.float64).max  # seconds; no time limit
     return p
 
 
@@ -259,6 +260,7 @@ def load_library():
     lib.tb200_last_qp_polish.argtypes = [C.c_void_p, _i32_p]
     lib.tb200_last_timing.argtypes = [C.c_void_p, C.POINTER(Timing)]
     lib.tb200_default_sqp_params.argtypes = [C.POINTER(SqpParams)]
+    lib.tb200_problem_set_sqp_params.argtypes = [C.c_void_p, C.POINTER(SqpParams)]
     lib.tb200_default_qp_settings.argtypes = [C.POINTER(QpSettings)]
     _LIB = lib
     return lib

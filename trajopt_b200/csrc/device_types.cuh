@@ -73,6 +73,7 @@ struct SqpParams {
   double trust_shrink_ratio, trust_expand_ratio, cnt_tolerance, max_merit_coeff_increases;
   double merit_coeff_increase_ratio, initial_merit_error_coeff, trust_box_size;
   int max_iter, max_qp_solver_failures, inflate_constraints_individually, pad;
+  double max_time;  // seconds; checked at the top of an SQP iteration (solve_kernel.cuh), DBL_MAX: no limit
 };
 
 // Everything a kernel needs; passed by value (pointers into device memory).
@@ -147,6 +148,9 @@ struct DevProblem {
   double* dbg;                 // [B][16] solver diagnostics of the last QP (residuals, polish residuals, rho, c)
   int* sched_state;            // [B] persistent SQP kernel: 0 ready, 1 running, 2 finished
   unsigned long long* sched_timers;  // [4] ns in QP steps, ns in evaluation steps, evaluation steps, claims
+  unsigned long long* clock_start;   // [1] %globaltimer ns at the start of the solve: the clock of sqp.max_time
+  int* sqp_top;                // [B] 1: the next QP of the trajectory begins a new SQP iteration (the time-limit check)
+  int* time_limited;           // [B] 1: the trajectory was ended by sqp.max_time (diagnostic)
   QpSettings qp;
   int qp_fast_passes;  // 1: short trajectories take the fused termination check and polish_passes (qp_cta_kernel.cuh)
   SqpParams sqp;

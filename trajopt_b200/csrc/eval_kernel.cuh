@@ -862,6 +862,7 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
     double* kv = p.cnt_viols + static_cast<size_t>(b) * p.n_cnts;
     double trust = p.trust[b];
     int accept = 0, finished = 0, status = 5;
+    int top = 0;  // the next QP begins a new SQP iteration (iter = 1 of a merit round, or ++iter): the time-limit check
     enum { NEXT_QP = 0, AFTER_LOOP = 1, PENALTY = 2 } go = NEXT_QP;
     if (ex.cast && p.lvs_overflow[b]) {
       // a step pair needed more LVS sub-segments than the candidate layout holds: the trajectory stops here and
@@ -871,6 +872,7 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
     } else if (mode == EVAL_INIT) {
       p.n_func_evals[b] = 1;
       accept = 2;  // rows of buffer 0 are the rows at x
+      top = 1;
     } else {
       p.n_qp_solves[b] += 1;
       double tr_old = 0, tr_model = 0, tr_new = 0;
@@ -943,6 +945,7 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
           p.sqp_iter[b] += 1;
           p.qp_failures[b] = 0;
           go = NEXT_QP;
+          top = 1;
         }
       }
       if (!finished && go == PENALTY) {  // optimizers.cpp:938-968
@@ -964,11 +967,13 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
           } else {
             p.sqp_iter[b] = 1;
             p.qp_failures[b] = 0;
+            top = 1;
           }
         }
       }
     }
     p.trust[b] = trust;
+    p.sqp_top[b] = top;  // (0 on a trust-region or QP-failure retry: no check inside the inner loop)
     if (mode == EVAL_STEP) p.qp_done[b] = 0;
     misc[0] = accept;
     if (finished) {

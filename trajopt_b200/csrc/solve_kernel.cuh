@@ -84,11 +84,41 @@ __device__ inline int claim_trajectory(const DevProblem& p, int* state, int tid)
   }
 }
 
+// sco's time limit (optimizers.cpp:738-753): checked where the reference checks it, at the top of every SQP iteration
+// (iter = 1 of each merit round and every ++iter, never on a trust-region or QP-failure retry); on the device that is
+// just before the QP that begins the iteration, so time spent waiting for a CTA counts.  Thread 0 reads the clock; a
+// trajectory past the limit ends with its last accepted iterate, OPT_CONVERGED when its constraints are within
+// cnt_tolerance (or it has none), else OPT_TIME_LIMIT.  A QP already running is not interrupted.  Returns (to every
+// thread) whether the trajectory ended here.
+__device__ inline bool time_limit_reached(const DevProblem& p, const int b, const int tid) {
+  __shared__ int s_stop;
+  if (tid == 0) {
+    int stop = 0;
+    if (p.sqp_top[b] && p.status[b] == 5) {
+      const double elapsed = static_cast<double>(global_ns() - *p.clock_start) * 1e-9;
+      if (elapsed > p.sqp.max_time) {
+        const double* kv = p.cnt_viols + static_cast<size_t>(b) * p.n_cnts;
+        double mx = -1e300;
+        for (int i = 0; i < p.n_cnts; ++i) mx = fmax(mx, kv[i]);
+        p.status[b] = (p.n_cnts == 0 || mx < p.sqp.cnt_tolerance) ? 0 : 3;  // OPT_CONVERGED | OPT_TIME_LIMIT
+        p.time_limited[b] = 1;
+        atomicSub(p.active_count, 1);
+        stop = 1;
+      }
+    }
+    s_stop = stop;
+  }
+  __syncthreads();
+  return s_stop != 0;  // (thread 0 writes it again only after the barriers of the next QP and evaluation steps)
+}
+constexpr double kNoTimeLimit = 1.7976931348623157e308;  // DBL_MAX, tb200_default_sqp_params
+
 template <int DD, int PAIR>
 __global__ void __launch_bounds__(kQpThreads, 1)
 solve_kernel(const __grid_constant__ DevProblem p, const __grid_constant__ EvalExtra ex, const __grid_constant__ SolveCtl ctl) {
   const int tid = threadIdx.x;
   const bool qp_only = ctl.mode == SOLVE_QP_ONLY;  // kernel-level entry point: one QP step per trajectory, no scheduler
+  const bool timed = !qp_only && p.sqp.max_time < kNoTimeLimit;  // (false for NaN too: such a limit never fires)
   for (int round = 0;; ++round) {
     const int bq = static_cast<int>(blockIdx.x) + round * static_cast<int>(gridDim.x);
     const int b = qp_only ? (bq < p.B ? bq : -1) : claim_trajectory(p, ctl.sched_state, tid);
@@ -96,6 +126,10 @@ solve_kernel(const __grid_constant__ DevProblem p, const __grid_constant__ EvalE
     unsigned long long t_qp = 0ull, t_ev = 0ull, n_ev = 0ull;
     bool finished = false;
     for (int step = 0; step < ctl.quantum && !finished; ++step) {
+      if (timed && time_limit_reached(p, b, tid)) {
+        finished = true;
+        break;
+      }
       const unsigned long long t0 = global_ns();
       // (a single call site: the QP solve stays inlined in the kernel, as tuned)
       qp_step<DD, PAIR>(p, b, ctl.x_override, ctl.trust_override, ctl.admm_iters_out, ctl.polish_out);

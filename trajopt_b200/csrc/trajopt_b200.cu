@@ -87,8 +87,8 @@ struct tb200_problem {
   DevBuf<int> fixed_vars;
   DevBuf<double> x, new_x, trust, merit_coeffs, cost_vals, cnt_viols, new_cost_vals, new_cnt_viols, model_cost_vals,
       model_cnt_viols, cart_err, cart_jac, coll_rows, rows, ws_x, ws_yb, scratch, ws_rho, x_tmp, trust_tmp, dbg, trace, factor_g, cast_scratch, soa;
-  DevBuf<unsigned long long> sched_timers;
-  DevBuf<int> sched_state;
+  DevBuf<unsigned long long> sched_timers, clock_start;
+  DevBuf<int> sched_state, sqp_top, time_limited;
   DevBuf<unsigned long long> coll_mask;
   DevBuf<int> status, sqp_iter, merit_round, qp_failures, qp_status, cur_buf, n_qp_solves, n_func_evals, n_admm_iters,
       active_count, row_ints, lists, ws_meta, tmp_iters, tmp_polish, trace_len, qp_done, lvs_overflow, link_chain, work_counter;
@@ -105,7 +105,7 @@ struct tb200_problem {
     x.release(); new_x.release(); trust.release(); merit_coeffs.release(); cost_vals.release(); cnt_viols.release();
     new_cost_vals.release(); new_cnt_viols.release(); model_cost_vals.release(); model_cnt_viols.release();
     cart_err.release(); cart_jac.release(); coll_rows.release(); rows.release(); ws_x.release(); ws_yb.release();
-    scratch.release(); ws_rho.release(); dbg.release(); trace.release(); trace_len.release(); factor_g.release(); cast_scratch.release(); soa.release(); lvs_overflow.release(); link_chain.release(); work_counter.release(); qp_done.release(); sched_state.release(); sched_timers.release(); x_tmp.release(); trust_tmp.release(); coll_mask.release(); status.release();
+    scratch.release(); ws_rho.release(); dbg.release(); trace.release(); trace_len.release(); factor_g.release(); cast_scratch.release(); soa.release(); lvs_overflow.release(); link_chain.release(); work_counter.release(); qp_done.release(); sched_state.release(); sched_timers.release(); clock_start.release(); sqp_top.release(); time_limited.release(); x_tmp.release(); trust_tmp.release(); coll_mask.release(); status.release();
     sqp_iter.release(); merit_round.release(); qp_failures.release(); qp_status.release(); cur_buf.release();
     n_qp_solves.release(); n_func_evals.release(); n_admm_iters.release(); active_count.release(); row_ints.release();
     lists.release(); ws_meta.release(); tmp_iters.release(); tmp_polish.release();
@@ -114,7 +114,7 @@ struct tb200_problem {
 
 extern "C" {
 
-const char* tb200_version(void) { return "trajopt_b200 0.1 (sm_90a)"; }
+const char* tb200_version(void) { return "trajopt_b200 0.2 (sm_90a)"; }
 const char* tb200_last_error(void) { return g_err.c_str(); }
 
 void tb200_default_sqp_params(tb200_sqp_params* p) {  // optimizers.hpp:92-135
@@ -133,6 +133,7 @@ void tb200_default_sqp_params(tb200_sqp_params* p) {  // optimizers.hpp:92-135
   p->trust_box_size = 0.1;
   p->inflate_constraints_individually = 1;
   p->reserved = 0;
+  p->max_time = std::numeric_limits<double>::max();  // no time limit
 }
 void tb200_osqp_order_qp_settings(tb200_qp_settings* s) {
   tb200_default_qp_settings(s);
@@ -617,6 +618,7 @@ int tb200_problem_create(const tb200_problem_desc* d, int device, tb200_problem*
   ALLOC(cur_buf, Bs); ALLOC(n_qp_solves, Bs); ALLOC(n_func_evals, Bs); ALLOC(n_admm_iters, Bs); ALLOC(active_count, 2);
   ALLOC(dbg, Bs * 16);
   ALLOC(sched_state, Bs); ALLOC(sched_timers, 8 + 2 * Bs);
+  ALLOC(clock_start, 1); ALLOC(sqp_top, Bs); ALLOC(time_limited, Bs);
   ALLOC(trace_len, Bs);
   ALLOC(x_tmp, Bs * N); ALLOC(trust_tmp, Bs); ALLOC(tmp_iters, Bs); ALLOC(tmp_polish, Bs);
 #undef ALLOC
@@ -635,6 +637,7 @@ int tb200_problem_create(const tb200_problem_desc* d, int device, tb200_problem*
   dp.rows = P->rows.p; dp.row_ints = P->row_ints.p; dp.lists = P->lists.p; dp.ws_x = P->ws_x.p; dp.ws_yb = P->ws_yb.p;
   dp.scratch = P->scratch.p; dp.ws_meta = P->ws_meta.p; dp.ws_rho = P->ws_rho.p; dp.dbg = P->dbg.p; dp.sched_state = P->sched_state.p; dp.sched_timers = P->sched_timers.p; dp.trace_len = P->trace_len.p; dp.trace = nullptr; dp.trace_cap = 0;
   dp.soa = P->soa.p;
+  dp.clock_start = P->clock_start.p; dp.sqp_top = P->sqp_top.p; dp.time_limited = P->time_limited.p;
   dp.factor_g = P->factor_g.p; dp.lvs_overflow = P->lvs_overflow.p; dp.qp_done = P->qp_done.p;
   P->ex.link_chain = P->link_chain.p;
   P->ex.work_counter = P->work_counter.p;
@@ -652,7 +655,7 @@ int tb200_problem_create(const tb200_problem_desc* d, int device, tb200_problem*
   dp.sqp = SqpParams{s.improve_ratio_threshold, s.min_trust_box_size, s.min_approx_improve, s.min_approx_improve_frac,
                      s.trust_shrink_ratio, s.trust_expand_ratio, s.cnt_tolerance, s.max_merit_coeff_increases,
                      s.merit_coeff_increase_ratio, s.initial_merit_error_coeff, s.trust_box_size, s.max_iter,
-                     s.max_qp_solver_failures, s.inflate_constraints_individually, 0};
+                     s.max_qp_solver_failures, s.inflate_constraints_individually, 0, s.max_time};
   int rc = tb200_problem_set_inputs(P, d->init_traj, d->cart_targets, d->obstacles);
   if (rc != TB200_OK) return rc;
   *out = guard.release();
@@ -672,7 +675,7 @@ int tb200_problem_set_sqp_params(tb200_problem* P, const tb200_sqp_params* s) {
   P->dp.sqp = SqpParams{s->improve_ratio_threshold, s->min_trust_box_size, s->min_approx_improve, s->min_approx_improve_frac,
                         s->trust_shrink_ratio, s->trust_expand_ratio, s->cnt_tolerance, s->max_merit_coeff_increases,
                         s->merit_coeff_increase_ratio, s->initial_merit_error_coeff, s->trust_box_size, s->max_iter,
-                        s->max_qp_solver_failures, s->inflate_constraints_individually, 0};
+                        s->max_qp_solver_failures, s->inflate_constraints_individually, 0, s->max_time};
   return TB200_OK;
 }
 
@@ -703,6 +706,7 @@ __global__ void reset_state_kernel(DevProblem p) {
     p.active_count[0] = p.B;
     p.active_count[1] = 0;
     for (int k = 0; k < 8; ++k) p.sched_timers[k] = (k == 4) ? ~0ull : 0ull;
+    *p.clock_start = global_ns();  // the time limit's clock: one start for the whole batch (DESIGN.md section 6)
   }
   if (b >= p.B) return;
   p.status[b] = 5;
@@ -724,6 +728,8 @@ __global__ void reset_state_kernel(DevProblem p) {
   p.sched_timers[8 + p.B + b] = 0ull;
   p.ws_rho[b] = p.qp.rho;
   p.trace_len[b] = 0;
+  p.sqp_top[b] = 0;  // (set by the initial evaluation)
+  p.time_limited[b] = 0;
 }
 
 cudaEvent_t getEvent(tb200_problem* P, size_t i) {
@@ -965,6 +971,17 @@ int tb200_debug_schedule(tb200_problem* P, unsigned long long* out) {
   const size_t B = P->dp.B;
   CK(cudaMemcpy(out, P->sched_timers.p + 4, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
   CK(cudaMemcpy(out + 1, P->sched_timers.p + 8, 2 * B * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+  return TB200_OK;
+}
+
+/* not part of the public header: the time limit of the last solve: *start_ns = %globaltimer at its start (the clock
+   the limit is measured on, comparable with tb200_debug_schedule's times), ended[b] = 1 when trajectory b was ended by
+   the limit */
+int tb200_debug_time_limit(tb200_problem* P, unsigned long long* start_ns, int32_t* ended) {
+  if (!P || !start_ns || !ended) return fail(TB200_ERR_INVALID, "null argument");
+  CK(cudaSetDevice(P->device));
+  CK(cudaMemcpy(start_ns, P->clock_start.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(ended, P->time_limited.p, static_cast<size_t>(P->dp.B) * sizeof(int), cudaMemcpyDeviceToHost));
   return TB200_OK;
 }
 

@@ -17,7 +17,8 @@ _COLL_KEYS = {"evaluator_type", "first_step", "last_step", "fixed_steps", "conta
               "coeffs", "dist_pen", "pairs"}
 _OPT_KEYS = ["improve_ratio_threshold", "min_trust_box_size", "min_approx_improve", "min_approx_improve_frac", "max_iter",
              "trust_shrink_ratio", "trust_expand_ratio", "cnt_tolerance", "max_merit_coeff_increases",
-             "merit_coeff_increase_ratio", "initial_merit_error_coeff", "inflate_constraints_individually", "trust_box_size"]
+             "merit_coeff_increase_ratio", "max_time", "initial_merit_error_coeff", "inflate_constraints_individually",
+             "trust_box_size"]
 
 
 def _only(params, allowed):  # ensure_only_members, problem_description.cpp:32-51
