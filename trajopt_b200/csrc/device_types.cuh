@@ -145,6 +145,7 @@ struct DevProblem {
   double* trace;               // [B][trace_cap][14] decision trace (same columns as the oracle's TraceEntry)
   int* trace_len;              // [B]
   int trace_cap, pad3;
+  int* qp_paths;               // [B] QpPath bits of every QP since the start of the solve (nullptr: not recorded)
   double* dbg;                 // [B][16] solver diagnostics of the last QP (residuals, polish residuals, rho, c)
   int* sched_state;            // [B] persistent SQP kernel: 0 ready, 1 running, 2 finished
   unsigned long long* sched_timers;  // [4] ns in QP steps, ns in evaluation steps, evaluation steps, claims

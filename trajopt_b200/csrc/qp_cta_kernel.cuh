@@ -1510,6 +1510,43 @@ __device__ __noinline__ bool assemble_factor(const QpCtx& q, const SysW& w) {
   return ok;
 }
 
+// The code paths of one QP solve (qp_solve_block), decided by the layout of the QP:
+//   use_reg:     the ADMM loop keeps the thread's rows of the factor in registers when the roles fit the CTA
+//   use_pinv:    short trajectories with their rows on chip use the partition-inverse form of the system (PinvPlan)
+//   fuse:        the partition-inverse block can end in the terms of a termination check ...
+//   fast_polish: ... and the polish refinement runs as polish_passes (else the generic passes of qp_solve_block)
+// regok: the register-resident solve may be used (blocks of <= 14); fast_passes: DevProblem::qp_fast_passes.
+struct QpPlan {
+  bool use_reg, use_pinv, fuse, fast_polish;
+};
+__host__ __device__ inline QpPlan qp_plan(bool regok, int pinv, int rows_smem, int M, int nb, bool fast_passes) {
+  QpPlan pl;
+  pl.use_reg = regok && solve_roles_fit(M, nb);
+  pl.use_pinv = regok && pinv && rows_smem;
+  pl.fuse = pl.use_pinv && fast_passes;
+  pl.fast_polish = pl.use_pinv && fast_passes && M * nb <= kQpThreads && solve_roles_fit(M, nb);
+  return pl;
+}
+// The code paths of a QP as bits (tb200_debug_qp_paths: ORed per trajectory over its QPs when recording is on)
+enum QpPath {
+  QPP_BLOCK_PINV = 1 << 0,      // ADMM blocks: admm_block_pinv
+  QPP_BLOCK_FAST = 1 << 1,      //              admm_block_fast
+  QPP_BLOCK_GENERIC = 1 << 2,   //              admm_block
+  QPP_BLOCK_SOA = 1 << 3,       //              admm_block_soa (rows in global memory)
+  QPP_FACTOR_GLOBAL = 1 << 4,   // the factor in this CTA's region of global memory
+  QPP_BAND_GLOBAL = 1 << 5,     // the objective band read from global memory
+  QPP_ROWS_GLOBAL = 1 << 6,     // the rows of the QP in global memory (more than row_cap)
+  QPP_FUSED_CHECK = 1 << 7,     // the termination checks take the residuals fused into admm_block_pinv
+  QPP_POLISH_FAST = 1 << 8,     // a polish was refined through polish_passes
+  QPP_POLISH_GENERIC = 1 << 9   // a polish was refined through the generic passes
+};
+// the ADMM block a plan runs (the choice of qp_solve_block's run_block)
+__host__ __device__ inline int qp_plan_block(const QpPlan& pl, int rows_smem) {
+  if (pl.use_pinv) return QPP_BLOCK_PINV;
+  if (!rows_smem) return QPP_BLOCK_SOA;
+  return pl.use_reg ? QPP_BLOCK_FAST : QPP_BLOCK_GENERIC;
+}
+
 struct QpOut {
   int status, iters, polish;
   double rho;
@@ -2720,15 +2757,13 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
   SysW sysw{false, st.sigma, rho};
   bool factor_ok = true;
 
-  // the ADMM loop keeps the thread's rows of the factor in registers when the roles fit the CTA (admm_block<.., true>)
-  const bool use_reg = REGOK && solve_roles_fit(q.M, NB);
-  // ... and short trajectories with their rows on chip use the partition-inverse form of the system (PinvPlan)
-  const bool use_pinv = REGOK && q.pinv && q.rows_smem;
+  // the ADMM block, the fused check and the polish refinement of this QP (QpPlan)
+  const QpPlan plan = qp_plan(REGOK, q.pinv, q.rows_smem, q.M, NB, fast_passes);
+  const bool use_reg = plan.use_reg;
+  const bool use_pinv = plan.use_pinv;
   using BlockFn = void (*)(const QpCtx&, double, int, int);
-  // fast_passes: the partition-inverse block can end in the terms of a termination check, and the polish refinement
-  // runs as polish_passes (else the generic passes of this function)
-  const bool fuse = use_pinv && fast_passes;
-  const bool fast_polish = use_pinv && fast_passes && q.Np <= kQpThreads && solve_roles_fit(q.M, NB);
+  const bool fuse = plan.fuse;
+  const bool fast_polish = plan.fast_polish;
   // q.tmp holds the fused check's partials of the current iterate: set by a block that computed them, cleared by every
   // factorisation (it reuses q.tmp)
   bool fused_chk = false;
@@ -3656,6 +3691,15 @@ __device__ __noinline__ void qp_step(const DevProblem& p, const int b, const dou
     }
     if (admm_iters_out) admm_iters_out[b] = res.iters;
     if (polish_out) polish_out[b] = res.polish;
+    if (p.qp_paths) {  // (off unless tb200_debug_enable_qp_paths)
+      const QpPlan pl = qp_plan(DD <= 7, q.pinv, q.rows_smem, q.M, NB, p.qp_fast_passes != 0);
+      int bits = qp_plan_block(pl, q.rows_smem) | (pl.fuse ? QPP_FUSED_CHECK : 0);
+      if (res.pol_factor_ok == 1) bits |= pl.fast_polish ? QPP_POLISH_FAST : QPP_POLISH_GENERIC;
+      if (FG || !S.factor_smem) bits |= QPP_FACTOR_GLOBAL;
+      if (!S.pband_smem) bits |= QPP_BAND_GLOBAL;
+      if (!rows_in_smem) bits |= QPP_ROWS_GLOBAL;
+      atomicOr(&p.qp_paths[b], bits);
+    }
     double* g = p.dbg + static_cast<size_t>(b) * 16;
     g[0] = res.status; g[1] = res.iters; g[2] = res.polish; g[3] = res.rho; g[4] = res.pri_res; g[5] = res.dua_res;
     g[6] = res.pol_pri; g[7] = res.pol_dua; g[8] = res.c; g[9] = res.pol_factor_ok; g[10] = res.rho_updates;

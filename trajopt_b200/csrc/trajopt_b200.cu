@@ -88,7 +88,7 @@ struct tb200_problem {
   DevBuf<double> x, new_x, trust, merit_coeffs, cost_vals, cnt_viols, new_cost_vals, new_cnt_viols, model_cost_vals,
       model_cnt_viols, cart_err, cart_jac, coll_rows, rows, ws_x, ws_yb, scratch, ws_rho, x_tmp, trust_tmp, dbg, trace, factor_g, cast_scratch, soa;
   DevBuf<unsigned long long> sched_timers, clock_start;
-  DevBuf<int> sched_state, sqp_top, time_limited;
+  DevBuf<int> sched_state, sqp_top, time_limited, qp_paths;
   DevBuf<unsigned long long> coll_mask;
   DevBuf<int> status, sqp_iter, merit_round, qp_failures, qp_status, cur_buf, n_qp_solves, n_func_evals, n_admm_iters,
       active_count, row_ints, lists, ws_meta, tmp_iters, tmp_polish, trace_len, qp_done, lvs_overflow, link_chain, work_counter;
@@ -105,7 +105,7 @@ struct tb200_problem {
     x.release(); new_x.release(); trust.release(); merit_coeffs.release(); cost_vals.release(); cnt_viols.release();
     new_cost_vals.release(); new_cnt_viols.release(); model_cost_vals.release(); model_cnt_viols.release();
     cart_err.release(); cart_jac.release(); coll_rows.release(); rows.release(); ws_x.release(); ws_yb.release();
-    scratch.release(); ws_rho.release(); dbg.release(); trace.release(); trace_len.release(); factor_g.release(); cast_scratch.release(); soa.release(); lvs_overflow.release(); link_chain.release(); work_counter.release(); qp_done.release(); sched_state.release(); sched_timers.release(); clock_start.release(); sqp_top.release(); time_limited.release(); x_tmp.release(); trust_tmp.release(); coll_mask.release(); status.release();
+    scratch.release(); ws_rho.release(); dbg.release(); trace.release(); trace_len.release(); factor_g.release(); cast_scratch.release(); soa.release(); lvs_overflow.release(); link_chain.release(); work_counter.release(); qp_done.release(); sched_state.release(); sched_timers.release(); clock_start.release(); sqp_top.release(); time_limited.release(); qp_paths.release(); x_tmp.release(); trust_tmp.release(); coll_mask.release(); status.release();
     sqp_iter.release(); merit_round.release(); qp_failures.release(); qp_status.release(); cur_buf.release();
     n_qp_solves.release(); n_func_evals.release(); n_admm_iters.release(); active_count.release(); row_ints.release();
     lists.release(); ws_meta.release(); tmp_iters.release(); tmp_polish.release();
@@ -754,6 +754,7 @@ int tb200_solve_batch_resident(tb200_problem* P) {
   cudaEvent_t e_begin = getEvent(P, 0), e_end = getEvent(P, 1), e_init0 = getEvent(P, 2), e_init1 = getEvent(P, 3);
   CK(cudaEventRecord(e_begin, st));
   reset_state_kernel<<<(dp.B + 127) / 128, 128, 0, st>>>(dp);
+  if (dp.qp_paths) CK(cudaMemsetAsync(dp.qp_paths, 0, dp.B * sizeof(int), st));
   // the initial evaluation + convexification of every trajectory: one CTA per trajectory (optimizers.cpp:761-783)
   CK(cudaEventRecord(e_init0, st));
   CK(cudaMemsetAsync(P->work_counter.p, 0, sizeof(int), st));
@@ -914,6 +915,7 @@ int tb200_qp_solve_batch(tb200_problem* P, const double* x, const double* trust,
   CK(cudaMemsetAsync(P->ws_meta.p, 0, B * 8 * sizeof(int), st));
   CK(cudaMemsetAsync(P->lvs_overflow.p, 0, B * sizeof(int), st));
   CK(cudaMemsetAsync(P->work_counter.p, 0, sizeof(int), st));
+  if (dp.qp_paths) CK(cudaMemsetAsync(dp.qp_paths, 0, B * sizeof(int), st));
   eval_kernel_for(P->D)<<<P->eval_grid, kEvalThreads, P->eval_smem, st>>>(dp, P->ex, EVAL_ONLY, P->x_tmp.p);
   SolveCtl ctl{};
   ctl.mode = SOLVE_QP_ONLY;  // one QP step per trajectory (one CTA each), no evaluation / decision
@@ -982,6 +984,47 @@ int tb200_debug_time_limit(tb200_problem* P, unsigned long long* start_ns, int32
   CK(cudaSetDevice(P->device));
   CK(cudaMemcpy(start_ns, P->clock_start.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
   CK(cudaMemcpy(ended, P->time_limited.p, static_cast<size_t>(P->dp.B) * sizeof(int), cudaMemcpyDeviceToHost));
+  return TB200_OK;
+}
+
+/* not part of the public header: record which code paths the QP solver takes (QpPath bits of qp_cta_kernel.cuh), on = 1,
+   or stop recording (on = 0, the default); then out[b] = the bits of every QP of trajectory b since the start of the last
+   tb200_solve_batch* / tb200_qp_solve_batch */
+int tb200_debug_enable_qp_paths(tb200_problem* P, int on) {
+  if (!P) return fail(TB200_ERR_INVALID, "null argument");
+  CK(cudaSetDevice(P->device));
+  if (on && !P->qp_paths.p) CK(P->qp_paths.alloc(static_cast<size_t>(P->dp.B)));
+  P->dp.qp_paths = on ? P->qp_paths.p : nullptr;
+  return TB200_OK;
+}
+/* not part of the public header, no device needed: the layout the QP step takes for a problem of n_steps waypoints of
+   n_dof joints whose QP rows span two waypoints (pair_rows) or one, with at most max_rows rows; a QP whose rows fit
+   shared memory, the default passes.  out[0] blocks M, [1] factor in global memory, [2] band in global memory,
+   [3] row_cap, [4] the ADMM block (QpPath bit), [5] 1: the fused check, [6] 1: polish_passes, [7] 1: partition
+   inverse planned (qp_smem_layout's pinv) */
+int tb200_debug_qp_layout(int n_steps, int n_dof, int pair_rows, int max_rows, int32_t* out) {
+  if (!out || n_steps < 1 || n_dof < 1 || n_dof > TB200_MAX_DOF || max_rows < 1) return fail(TB200_ERR_INVALID, "bad argument");
+  const int N = n_steps * n_dof, nb = 2 * n_dof;
+  const int CN = pair_rows ? std::max(2 * n_dof, 3) : std::max(n_dof, 3);
+  const bool fg = n_dof > 8;  // = FG of qp_step
+  const QpSmem s = qp_smem_layout(N, nb, qp_row_stride(CN), CN, max_rows, fg);
+  const int M = qp_block_count(N, nb);
+  const QpPlan pl = qp_plan(n_dof <= 7, s.pinv, 1, M, nb, true);
+  out[0] = M;
+  out[1] = (fg || !s.factor_smem) ? 1 : 0;
+  out[2] = s.pband_smem ? 0 : 1;
+  out[3] = s.row_cap;
+  out[4] = qp_plan_block(pl, 1);
+  out[5] = pl.fuse ? 1 : 0;
+  out[6] = pl.fast_polish ? 1 : 0;
+  out[7] = s.pinv;
+  return TB200_OK;
+}
+int tb200_debug_qp_paths(tb200_problem* P, int32_t* out) {
+  if (!P || !out) return fail(TB200_ERR_INVALID, "null argument");
+  if (!P->dp.qp_paths) return fail(TB200_ERR_INVALID, "QP path recording is off (tb200_debug_enable_qp_paths)");
+  CK(cudaSetDevice(P->device));
+  CK(cudaMemcpy(out, P->qp_paths.p, static_cast<size_t>(P->dp.B) * sizeof(int), cudaMemcpyDeviceToHost));
   return TB200_OK;
 }
 
