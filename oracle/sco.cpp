@@ -443,6 +443,12 @@ QPResult qp_solve(const QP& qp, const QPSettings& s, const QPWarmStart* warm) {
   w.q = qp.q;
   w.l = qp.l;
   w.u = qp.u;
+  // bounds beyond OSQP_INFTY (+-inf included) mean "none": clamp them as the device kernels do, so that no inf
+  // reaches a product (inf * 0 = NaN in the polish right-hand side and the infeasibility certificate)
+  for (int r = 0; r < m; ++r) {
+    w.l[r] = std::max(w.l[r], -OSQP_INFTY);
+    w.u[r] = std::min(w.u[r], OSQP_INFTY);
+  }
   if (s.scaling > 0)
     ruizScale(w, s.scaling);
   else {
@@ -599,7 +605,9 @@ QPResult qp_solve(const QP& qp, const QPSettings& s, const QPWarmStart* warm) {
         updateInfo();
         status = checkTermination(false);
         if (status != QP_UNSOLVED) return;
-        bool try_early = s.early_polish_every > 0 && iter >= s.early_polish_from && (iter % s.early_polish_every == 0);
+        // the early polish is a polish: without polishing, ADMM alone must meet its tolerances (as in both kernels)
+        bool try_early = s.polishing && s.early_polish_every > 0 && iter >= s.early_polish_from &&
+                         (iter % s.early_polish_every == 0);
         if (try_early && s.early_polish_stable) {
           // only when the active-set guess has settled (same as at the previous test) and has not failed before
           const uint64_t h = guessHash();

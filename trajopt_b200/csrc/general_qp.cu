@@ -4,8 +4,8 @@
 // solved by the same OSQP-equivalent ADMM as the trajectory QPs (Ruiz equilibration, rho_eq = 1e3 rho on equality rows,
 // alpha = 1.6, termination + infeasibility certificates every check_termination iterations, adaptive rho, polish with KKT
 // verification and ADMM continuation — DESIGN.md section 6), restated for an arbitrary dense P and A: one CTA per QP,
-// the reduced KKT matrix  K = P + sigma I + A' diag(rho) A  inverted explicitly (Gauss-Jordan, K is SPD) so that an ADMM
-// iteration is three dense products.  This is the compatibility surface (a sco::Model::optimize() call at a time, what
+// the reduced KKT matrix  K = P + sigma I + A' diag(rho) A  factored by a dense Cholesky (K is SPD) so that an ADMM
+// iteration is dense products and two triangular solves.  This is the compatibility surface (a sco::Model::optimize() call at a time, what
 // trajopt_sco's own SQP loop issues); the batched trajectory path does not go through it.
 #include <cuda_runtime.h>
 
@@ -20,6 +20,7 @@ constexpr int kThreads = 256;
 constexpr double kInf = 1e30, kMinScaling = 1e-4, kMaxScaling = 1e4;
 constexpr double kRhoMin = 1e-6, kRhoMax = 1e6, kRhoTol = 1e-4, kRhoEq = 1e3, kVerifyTol = 1e-9;
 constexpr int kVerifyRounds = 3;
+constexpr long long kMaxDenseEntries = 2147483647LL;
 enum { S_UNSOLVED = 0, S_SOLVED = 1, S_SOLVED_INACC = 2, S_PINF = 3, S_PINF_INACC = 4, S_DINF = 5, S_DINF_INACC = 6, S_MAXITER = 7, S_NONCVX = 8 };
 
 struct GqDev {
@@ -60,7 +61,6 @@ struct Red {
 __global__ void __launch_bounds__(kThreads, 1) general_qp_kernel(const __grid_constant__ GqDev g) {
   __shared__ double s_red[kThreads / 32];
   __shared__ unsigned long long s_h[kThreads / 32];
-  __shared__ int s_flag;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, b = blockIdx.x;
   const int n = g.n, m = g.m;
   const tb200_qp_settings& st = g.st;
@@ -74,9 +74,9 @@ __global__ void __launch_bounds__(kThreads, 1) general_qp_kernel(const __grid_co
   };
   double* Ps = take(static_cast<size_t>(n) * n);  // scaled P (full symmetric)
   double* As = take(static_cast<size_t>(m) * n);  // scaled A (row major)
-  double* K = take(static_cast<size_t>(n) * n);   // inverse of the current reduced KKT matrix
+  double* K = take(static_cast<size_t>(n) * n);   // Cholesky factor of the current reduced KKT matrix (L and L')
   double *qs = take(n), *D = take(n), *x = take(n), *xt = take(n), *rhs = take(n), *tmpn = take(n), *Px = take(n), *Aty = take(n),
-         *dx = take(n), *xq = take(n), *rd = take(n), *stepv = take(n), *colk = take(n), *rowk = take(n), *sx = take(n);
+         *dx = take(n), *xq = take(n), *rd = take(n), *stepv = take(n), *colk = take(n), *sx = take(n);
   double *ls = take(m), *us = take(m), *E = take(m), *rho_vec = take(m), *z = take(m), *y = take(m), *zt = take(m), *tmpm = take(m),
          *Ax = take(m), *dy = take(m), *wact = take(m), *bb = take(m), *act = take(m), *yq = take(m), *sz = take(m), *sy = take(m);
   const double* P0 = g.P + static_cast<size_t>(b) * n * n;
@@ -108,8 +108,12 @@ __global__ void __launch_bounds__(kThreads, 1) general_qp_kernel(const __grid_co
     }
     __syncthreads();
   };
-  // K <- (Ps + sig I + As' diag(wts) As)^-1 ; false when the matrix is not positive definite
-  auto assemble_invert = [&](double sig, const double* wts) -> bool {
+  // K <- Cholesky factor of Ps + sig I + As' diag(wts) As, L in the lower triangle and L' in the upper (so that both
+  // triangular solves walk rows: coalesced); false when the matrix is not positive definite.  A factor, not an explicit
+  // inverse: the ADMM matrix (rho_eq = 1e3 rho up to 1e6) and the polish matrix (1/delta = 1e6 on the active rows) reach
+  // condition numbers of 1e12 and more on penalty QPs whose P is singular on the slacks, where an explicit inverse loses
+  // every digit and the Cholesky solve stays backward stable.
+  auto assemble_factor = [&](double sig, const double* wts) -> bool {
     for (int e = tid; e < n * n; e += kThreads) {
       const int i = e / n, j = e % n;
       double s = Ps[e] + (i == j ? sig : 0.0);
@@ -119,30 +123,46 @@ __global__ void __launch_bounds__(kThreads, 1) general_qp_kernel(const __grid_co
       }
       K[e] = s;
     }
-    if (tid == 0) s_flag = 0;
     __syncthreads();
-    for (int k = 0; k < n; ++k) {  // in-place Gauss-Jordan without pivoting (SPD)
+    for (int k = 0; k < n; ++k) {  // right-looking, on the upper triangle: row k of U = L' is column k of L
       const double piv = K[static_cast<size_t>(k) * n + k];
-      if (!(piv > 0.0)) {
-        s_flag = 1;  // (every thread reads the same pivot: a benign identical write)
-      }
-      const double ip = 1.0 / piv;
-      for (int j = tid; j < n; j += kThreads) {
-        colk[j] = K[static_cast<size_t>(j) * n + k];
-        rowk[j] = K[static_cast<size_t>(k) * n + j] * ip;
-      }
+      __syncthreads();            // every thread has read the pivot before row k is overwritten
+      if (!(piv > 0.0)) return false;  // every thread read the same pivot: a uniform exit
+      const double lkk = sqrt(piv), il = 1.0 / lkk;
+      for (int j = k + tid; j < n; j += kThreads) K[static_cast<size_t>(k) * n + j] = j == k ? lkk : K[static_cast<size_t>(k) * n + j] * il;
       __syncthreads();
-      for (int e = tid; e < n * n; e += kThreads) {
-        const int i = e / n, j = e % n;
-        double v;
-        if (i == k) v = (j == k) ? ip : rowk[j];
-        else if (j == k) v = -colk[i] * ip;
-        else v = K[e] - colk[i] * rowk[j];
-        K[e] = v;
+      const int r = n - k - 1;
+      for (int e = tid; e < r * r; e += kThreads) {
+        const int i = k + 1 + e / r, j = k + 1 + e % r;
+        if (j >= i) K[static_cast<size_t>(i) * n + j] -= K[static_cast<size_t>(k) * n + i] * K[static_cast<size_t>(k) * n + j];
       }
       __syncthreads();
     }
-    return s_flag == 0;
+    for (int e = tid; e < n * n; e += kThreads) {  // mirror: K[i][j] = L[i][j] below the diagonal
+      const int i = e / n, j = e % n;
+      if (i > j) K[e] = K[static_cast<size_t>(j) * n + i];
+    }
+    __syncthreads();
+    return true;
+  };
+  // out = (L L')^-1 in with the factor of assemble_factor; in and out distinct, colk is scratch
+  auto chol_solve = [&](const double* in, double* out) {
+    for (int i = tid; i < n; i += kThreads) colk[i] = in[i];
+    __syncthreads();
+    for (int k = 0; k < n; ++k) {  // L w = in: colk[k] is final once step k - 1 is done
+      const double wk = colk[k] / K[static_cast<size_t>(k) * n + k];
+      for (int i = k + 1 + tid; i < n; i += kThreads) colk[i] -= K[static_cast<size_t>(k) * n + i] * wk;
+      if (tid == 0) out[k] = wk;
+      __syncthreads();
+    }
+    for (int i = tid; i < n; i += kThreads) colk[i] = out[i];
+    __syncthreads();
+    for (int k = n - 1; k >= 0; --k) {  // L' x = w: row k of L holds column k of L'
+      const double xk = colk[k] / K[static_cast<size_t>(k) * n + k];
+      for (int i = tid; i < k; i += kThreads) colk[i] -= K[static_cast<size_t>(k) * n + i] * xk;
+      if (tid == 0) out[k] = xk;
+      __syncthreads();
+    }
   };
 
   // ---- copy + Ruiz equilibration (scale_data of OSQP; same passes as the trajectory kernel's qp_scale) --------------
@@ -224,7 +244,7 @@ __global__ void __launch_bounds__(kThreads, 1) general_qp_kernel(const __grid_co
   bool early_verified = false;
   unsigned long long prev_guess = 0ull, failed_guess = 0ull, pending_guess = 0ull;
   bool have_prev = false, have_failed = false;
-  if (!assemble_invert(st.sigma, rho_vec)) status = S_NONCVX;
+  if (!assemble_factor(st.sigma, rho_vec)) status = S_NONCVX;
 
   auto update_info = [&]() {
     A_mv(x, Ax);
@@ -340,7 +360,7 @@ __global__ void __launch_bounds__(kThreads, 1) general_qp_kernel(const __grid_co
     }
     for (int i = tid; i < n; i += kThreads) xq[i] = 0.0;
     __syncthreads();
-    if (!assemble_invert(st.delta, wact)) return false;
+    if (!assemble_factor(st.delta, wact)) return false;
     for (int it = 0; it <= st.polish_refine_iter; ++it) {
       sym_mv(Ps, xq, Px);
       At_mv(yq, Aty);
@@ -350,7 +370,7 @@ __global__ void __launch_bounds__(kThreads, 1) general_qp_kernel(const __grid_co
       At_mv(tmpm, tmpn);
       for (int i = tid; i < n; i += kThreads) rd[i] = -(Px[i] + qs[i] + Aty[i]) - tmpn[i];
       __syncthreads();
-      sym_mv(K, rd, stepv);
+      chol_solve(rd, stepv);
       for (int i = tid; i < n; i += kThreads) xq[i] += stepv[i];
       __syncthreads();
       A_mv(xq, Ax);
@@ -397,7 +417,7 @@ __global__ void __launch_bounds__(kThreads, 1) general_qp_kernel(const __grid_co
       At_mv(tmpm, rhs);
       for (int i = tid; i < n; i += kThreads) rhs[i] += st.sigma * x[i] - qs[i];
       __syncthreads();
-      sym_mv(K, rhs, xt);
+      chol_solve(rhs, xt);
       A_mv(xt, zt);
       for (int i = tid; i < n; i += kThreads) {
         const double xn = st.alpha * xt[i] + (1.0 - st.alpha) * x[i];
@@ -438,7 +458,7 @@ __global__ void __launch_bounds__(kThreads, 1) general_qp_kernel(const __grid_co
           failed_guess = pending_guess;
           have_failed = true;
           update_info();
-          if (!assemble_invert(st.sigma, rho_vec)) {
+          if (!assemble_factor(st.sigma, rho_vec)) {
             status = S_NONCVX;
             break;
           }
@@ -466,7 +486,7 @@ __global__ void __launch_bounds__(kThreads, 1) general_qp_kernel(const __grid_co
         if (rho_new > rho * st.adaptive_rho_tolerance || rho_new < rho / st.adaptive_rho_tolerance) {
           rho = rho_new;
           set_rho();
-          if (!assemble_invert(st.sigma, rho_vec)) {
+          if (!assemble_factor(st.sigma, rho_vec)) {
             status = S_NONCVX;
             break;
           }
@@ -492,12 +512,12 @@ __global__ void __launch_bounds__(kThreads, 1) general_qp_kernel(const __grid_co
     }
     ++round;
     eps_scale *= 0.1;
-    if (!assemble_invert(st.sigma, rho_vec)) {
+    if (!assemble_factor(st.sigma, rho_vec)) {
       status = S_NONCVX;
       break;
     }
   }
-  (void)sx; (void)sz; (void)sy; (void)colk; (void)rowk;
+  (void)sx; (void)sz; (void)sy;
   // ---- unscale and store ---------------------------------------------------------------------------------------------
   const double* xs = polish > 0 ? xq : x;
   const double* ys = polish > 0 ? yq : y;
@@ -527,6 +547,9 @@ int tb200_qp_solve_general(const tb200_qp_general* qp, const tb200_qp_settings* 
   const int n = qp->n, m = qp->m, B = qp->batch < 1 ? 1 : qp->batch;
   if (n < 1 || m < 0) return fail(TB200_ERR_INVALID, "n must be >= 1 and m >= 0");
   if (!qp->P || !qp->q || (m > 0 && (!qp->A || !qp->l || !qp->u))) return fail(TB200_ERR_INVALID, "null QP data");
+  // the kernel indexes P, K and A with 32-bit n * n and m * n (one CTA per QP: far beyond any size it is meant for)
+  if (static_cast<long long>(n) * n > kMaxDenseEntries || static_cast<long long>(m) * n > kMaxDenseEntries)
+    return fail(TB200_ERR_UNSUPPORTED, "general QP too large: n * n and m * n must each be at most 2^31 - 1");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
     return fail(TB200_ERR_NO_DEVICE, "no CUDA device: trajopt_b200 has no CPU fallback");
@@ -541,7 +564,7 @@ int tb200_qp_solve_general(const tb200_qp_general* qp, const tb200_qp_settings* 
   if (settings) st = *settings;
   else tb200_default_qp_settings(&st);
   const size_t nn = static_cast<size_t>(n) * n, mn = static_cast<size_t>(m) * n;
-  const size_t ws = 2 * (nn + 2) + (mn + 2) + 15 * (static_cast<size_t>(n) + 2) + 16 * (static_cast<size_t>(m) + 2);
+  const size_t ws = 2 * (nn + 2) + (mn + 2) + 14 * (static_cast<size_t>(n) + 2) + 16 * (static_cast<size_t>(m) + 2);
   double *dP = nullptr, *dq = nullptr, *dA = nullptr, *dl = nullptr, *du = nullptr, *dws = nullptr, *dx = nullptr, *dy = nullptr;
   int* dint = nullptr;
   auto release = [&]() {
