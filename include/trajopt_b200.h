@@ -30,7 +30,7 @@ extern "C" {
 #endif
 
 #define TB200_VERSION_MAJOR 0
-#define TB200_VERSION_MINOR 2
+#define TB200_VERSION_MINOR 3
 #define TB200_MAX_DOF 16      /* joints per manipulator group (7 single arm, 14 dual arm) */
 #define TB200_MAX_STEPS 64    /* waypoints per trajectory */
 #define TB200_MIN_CAST_ROWS_PER_PAIR 128  /* continuous collision evaluators: lower / upper limit of the active contacts */
@@ -205,6 +205,13 @@ typedef struct tb200_problem_desc {
   const double* obstacles;  /* (x,y,z,r) in the scene root frame */
   tb200_sqp_params sqp;
   tb200_qp_settings qp;
+  /* Multi-start solves (not in the reference; DESIGN.md section 4.1).  group_size G >= 2: trajectories [g*G, (g+1)*G) are
+   * G seeds of problem g (batch % G == 0); 0 or 1: no groups.  group_stop 1: a seed that ends OPT_CONVERGED by its own
+   * SQP ends its running siblings at their next SQP iteration top, under the time-limit rule (last accepted iterate;
+   * OPT_CONVERGED when its constraints are within cnt_tolerance, else OPT_TIME_LIMIT); 0: every seed runs to its end.
+   * The best seed of every group is selected on the device (tb200_fetch_group_results). */
+  int32_t group_size;
+  int32_t group_stop;
 } tb200_problem_desc;
 
 /* Caller-owned result buffers = sco::OptResults per trajectory (optimizers.hpp:40-59).
@@ -311,6 +318,24 @@ int tb200_solve_batch(tb200_problem* p, tb200_results* out);
  * device until tb200_fetch_results.  Used for the HBM-resident bench leg. */
 int tb200_solve_batch_resident(tb200_problem* p);
 int tb200_fetch_results(tb200_problem* p, tb200_results* out);
+
+/* Replace group_size / group_stop of an existing problem (same rules as in tb200_problem_desc).  Takes effect at the
+ * next solve. */
+int tb200_problem_set_groups(tb200_problem* p, int32_t group_size, int32_t group_stop);
+
+/* Per-group results of the last solve; NG = batch / group_size groups (without groups every trajectory is its own
+ * group, NG = batch).  The best seed of a group is the minimum of the key
+ *   (status != OPT_CONVERGED, status != OPT_CONVERGED ? max(cnt_viols) : 0, total_cost, batch index)
+ * with a NaN read as +inf.  Any pointer may be NULL to skip that output. */
+typedef struct tb200_group_results {
+  int32_t* best;            /* [NG] batch index of the best seed */
+  int32_t* status;          /* [NG] its status */
+  double* total_cost;       /* [NG] its total cost */
+  double* x;                /* [NG][T][D] its trajectory */
+  int32_t* n_converged;     /* [NG] seeds of the group that ended OPT_CONVERGED */
+  int32_t* ended_by;        /* [batch] per trajectory: 0 its own SQP, 1 the time limit (max_time), 2 its group */
+} tb200_group_results;
+int tb200_fetch_group_results(tb200_problem* p, tb200_group_results* out);
 
 /* Kernel-level entry points for parity tests.
  * x: host [B][T][D].  Equivalent of costs[i]->convex/value + cnts[i]->convex/violation

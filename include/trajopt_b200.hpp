@@ -242,6 +242,11 @@ struct ProblemConstructionInfo {
   DblVec obstacles;  // static world spheres (x, y, z, r): [B][O][4] or [O][4]
   int n_obstacles = 0;
   bool obstacles_per_problem = true;
+  // Multi-start (not in the reference): batch = problems * seeds_per_problem; trajectories [p*G, (p+1)*G) are the seeds
+  // of problem p (they normally differ only in init_info).  stop_seeds_on_converged: once a seed converges, its
+  // siblings end at their next SQP iteration top (tb200_problem_desc.group_stop).  OptimizeProblemMultiStart.
+  int seeds_per_problem = 1;
+  bool stop_seeds_on_converged = false;
 };
 
 inline void JointTermInfoBase::hatch(Flat& flat, const ProblemConstructionInfo& pci) const {
@@ -426,6 +431,8 @@ inline std::shared_ptr<FlatProblem> FlattenProblem(const ProblemConstructionInfo
   d.sqp.inflate_constraints_individually = p.inflate_constraints_individually ? 1 : 0;
   d.sqp.reserved = 0;
   d.sqp.max_time = p.max_time;
+  d.group_size = pci.seeds_per_problem;
+  d.group_stop = pci.stop_seeds_on_converged ? 1 : 0;
   return fp;
 }
 
@@ -443,6 +450,7 @@ public:
   int GetNumSteps() const { return flat_->desc.n_steps; }
   int GetNumDOF() const { return flat_->desc.robot.n_dof; }
   int GetBatch() const { return flat_->desc.batch; }
+  int GetSeedsPerProblem() const { return flat_->desc.group_size > 1 ? flat_->desc.group_size : 1; }
   const DblVec& GetInitTraj() const { return flat_->init_traj; }
   const tb200_sqp_params& sqpParams() const { return flat_->desc.sqp; }  // = pci.opt_info
   int getNumCosts() const { return layout_.n_costs; }
@@ -502,6 +510,36 @@ inline std::vector<sco::OptResults> OptimizeProblem(TrajOptProb& prob) {
   p.improve_ratio_threshold = .2;
   p.initial_merit_error_coeff = 20;
   return OptimizeWithParams(prob, p);
+}
+
+// One problem of a multi-start solve (ProblemConstructionInfo::seeds_per_problem): its best seed and what every seed did.
+struct MultiStartResult {
+  int best = -1;                            // batch index of the best seed
+  sco::OptResults result;                   // the best seed's results
+  std::vector<sco::OptStatus> seed_status;  // status of every seed of the problem, in batch order
+};
+
+// Every problem of a multi-start batch, with the given parameters: the seeds are solved together (siblings stopped on the
+// device when pci.stop_seeds_on_converged) and the best seed of each problem is selected on the device by the key of
+// tb200_group_results (converged first, then the smallest constraint violation, then total cost, then index).
+inline std::vector<MultiStartResult> OptimizeProblemMultiStart(TrajOptProb& prob, const tb200_sqp_params& params) {
+  const std::vector<sco::OptResults> seeds = OptimizeWithParams(prob, params);
+  const int G = prob.GetSeedsPerProblem(), NG = prob.GetBatch() / G;
+  std::vector<int32_t> best(NG);
+  tb200_group_results g{};
+  g.best = best.data();
+  if (tb200_fetch_group_results(prob.handle(), &g) != TB200_OK) throw std::runtime_error(tb200_last_error());
+  std::vector<MultiStartResult> out(NG);
+  for (int p = 0; p < NG; ++p) {
+    out[p].best = best[p];
+    out[p].result = seeds[best[p]];
+    for (int k = 0; k < G; ++k) out[p].seed_status.push_back(seeds[p * G + k].status);
+  }
+  return out;
+}
+// ... with the problem description's own parameters (pci.opt_info)
+inline std::vector<MultiStartResult> OptimizeProblemMultiStart(TrajOptProb& prob) {
+  return OptimizeProblemMultiStart(prob, prob.sqpParams());
 }
 
 }  // namespace trajopt

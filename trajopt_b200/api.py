@@ -31,6 +31,8 @@ class Problem:
             raise RuntimeError(f"tb200_problem_create failed ({rc}): {self.lib.tb200_last_error().decode()}")
         self.layout = capi.Layout()
         self._check(self.lib.tb200_problem_layout(self.handle, C.byref(self.layout)))
+        self.group_size = max(desc.c.group_size, 1)
+        self._solved_group_size = None
 
     def _check(self, rc):
         if rc != 0:
@@ -57,6 +59,24 @@ class Problem:
         """Replace the optimizer parameters (a capi.SqpParams, e.g. with a new max_time) for the next solves."""
         self._check(self.lib.tb200_problem_set_sqp_params(self.handle, C.byref(sqp)))
 
+    def set_groups(self, group_size, group_stop=0):
+        """Multi-start: trajectories [g*G, (g+1)*G) are G seeds of problem g (G = 0 or 1: no groups); group_stop 1
+        ends the siblings of a seed that converges at their next SQP iteration top.  For the next solves."""
+        self._check(self.lib.tb200_problem_set_groups(self.handle, group_size, group_stop))
+        self.group_size = max(int(group_size), 1)
+
+    def group_results(self):
+        """Per group of the last solve: the best seed's batch index, status, total cost and x, and how many seeds
+        converged; per trajectory: ended_by (0 its own SQP, 1 the time limit, 2 its group)."""
+        d = self.desc
+        NG = d.B // (self._solved_group_size or 1)  # (before any solve the library refuses)
+        out = dict(best=np.zeros(NG, np.int32), status=np.zeros(NG, np.int32), total_cost=np.zeros(NG),
+                   x=np.zeros((NG, d.T, d.D)), n_converged=np.zeros(NG, np.int32), ended_by=np.zeros(d.B, np.int32))
+        r = capi.GroupResults(_ip(out["best"]), _ip(out["status"]), _dp(out["total_cost"]), _dp(out["x"]),
+                              _ip(out["n_converged"]), _ip(out["ended_by"]))
+        self._check(self.lib.tb200_fetch_group_results(self.handle, C.byref(r)))
+        return out
+
     def _results(self):
         L, d = self.layout, self.desc
         return capi.alloc_results(d.B, d.T, d.D, L.n_costs, L.n_cnts)
@@ -64,11 +84,13 @@ class Problem:
     def solve(self):
         """BasicTrustRegionSQP::optimize() for the whole batch; host buffers in and out."""
         buf, res = self._results()
+        self._solved_group_size = self.group_size
         self._check(self.lib.tb200_solve_batch(self.handle, C.byref(res)))
         buf["timing"] = self.timing()
         return buf
 
     def solve_resident(self):
+        self._solved_group_size = self.group_size
         self._check(self.lib.tb200_solve_batch_resident(self.handle))
 
     def fetch(self):
@@ -126,11 +148,19 @@ class Problem:
         return out
 
 
-def solve(desc, device=0):
-    """One-shot: create, solve, destroy."""
+def solve(desc, device=0, group_size=None, group_stop=None):
+    """One-shot: create, solve, destroy.  With group_size (and group_stop) the solve is a multi-start one
+    (Problem.set_groups; None keeps the description's own settings) and the result gains a "groups" dict
+    (Problem.group_results)."""
     p = Problem(desc, device)
     try:
-        return p.solve()
+        if group_size is not None or group_stop is not None:
+            p.set_groups(desc.c.group_size if group_size is None else group_size,
+                         desc.c.group_stop if group_stop is None else group_stop)
+        out = p.solve()
+        if group_size is not None:
+            out["groups"] = p.group_results()
+        return out
     finally:
         p.close()
 

@@ -77,7 +77,8 @@ class ProblemDescC(C.Structure):
                 ("n_fixed_timesteps", C.c_int32), ("terms", C.POINTER(Term)), ("fixed_timesteps", _i32_p),
                 ("n_fixed_dofs", C.c_int32), ("n_cart_targets", C.c_int32), ("fixed_dofs", _i32_p),
                 ("init_traj", _dbl_p), ("cart_targets", _dbl_p), ("n_obstacles", C.c_int32),
-                ("obstacles_per_traj", C.c_int32), ("obstacles", _dbl_p), ("sqp", SqpParams), ("qp", QpSettings)]
+                ("obstacles_per_traj", C.c_int32), ("obstacles", _dbl_p), ("sqp", SqpParams), ("qp", QpSettings),
+                ("group_size", C.c_int32), ("group_stop", C.c_int32)]
 
 
 class QpGeneral(C.Structure):
@@ -89,6 +90,11 @@ class QpGeneral(C.Structure):
 class Results(C.Structure):
     _fields_ = [("x", _dbl_p), ("status", _i32_p), ("total_cost", _dbl_p), ("cost_vals", _dbl_p),
                 ("cnt_viols", _dbl_p), ("n_qp_solves", _i32_p), ("n_func_evals", _i32_p), ("n_admm_iters", _i32_p)]
+
+
+class GroupResults(C.Structure):
+    _fields_ = [("best", _i32_p), ("status", _i32_p), ("total_cost", _dbl_p), ("x", _dbl_p), ("n_converged", _i32_p),
+                ("ended_by", _i32_p)]
 
 
 class ConvexifyOut(C.Structure):
@@ -156,7 +162,9 @@ class ProblemDesc:
     """Python-side owner of a tb200_problem_desc: keeps every buffer alive."""
 
     def __init__(self, robot, n_steps, terms, init_traj, fixed_timesteps=(), fixed_dofs=(), cart_targets=None,
-                 obstacles=None, obstacles_per_traj=True, sqp=None, qp=None):
+                 obstacles=None, obstacles_per_traj=True, sqp=None, qp=None, group_size=0, group_stop=0):
+        """group_size G >= 2: trajectories [g*G, (g+1)*G) are G seeds of problem g; group_stop 1: the siblings of a seed
+        that converges stop at their next SQP iteration top (include/trajopt_b200.h)."""
         self.robot_spec = robot
         init_traj = np.ascontiguousarray(init_traj, dtype=np.float64)
         assert init_traj.ndim == 3 and init_traj.shape[1] == n_steps and init_traj.shape[2] == robot["n_dof"]
@@ -198,16 +206,22 @@ class ProblemDesc:
             d.obstacles = _dp(self.obstacles)
         d.sqp = sqp if sqp is not None else default_sqp_params()
         d.qp = qp if qp is not None else default_qp_settings()
+        d.group_size, d.group_stop = group_size, group_stop
         self.c = d
 
     def slice(self, b0, b1):
-        """A description holding only trajectories [b0, b1) (for sharding / small oracle runs)."""
+        """A description holding only trajectories [b0, b1) (for sharding / small oracle runs).  With groups the cut
+        must fall on group boundaries: a group is never split."""
+        G = max(self.c.group_size, 1)
+        if b0 % G or b1 % G:
+            raise ValueError(f"[{b0}, {b1}) splits a group of {G} seeds")
         return ProblemDesc(self.robot_spec, self.T, self.terms, self.init_traj[b0:b1],
                            fixed_timesteps=self._fixed_t, fixed_dofs=self._fixed_d,
                            cart_targets=None if self.cart_targets is None else self.cart_targets[b0:b1],
                            obstacles=None if self.obstacles is None else
                            (self.obstacles[b0:b1] if self.c.obstacles_per_traj else self.obstacles),
-                           obstacles_per_traj=bool(self.c.obstacles_per_traj), sqp=self.c.sqp, qp=self.c.qp)
+                           obstacles_per_traj=bool(self.c.obstacles_per_traj), sqp=self.c.sqp, qp=self.c.qp,
+                           group_size=self.c.group_size, group_stop=self.c.group_stop)
 
 
 def alloc_results(B, T, D, n_costs, n_cnts):
@@ -262,6 +276,8 @@ def load_library():
     lib.tb200_default_sqp_params.argtypes = [C.POINTER(SqpParams)]
     lib.tb200_problem_set_sqp_params.argtypes = [C.c_void_p, C.POINTER(SqpParams)]
     lib.tb200_default_qp_settings.argtypes = [C.POINTER(QpSettings)]
+    lib.tb200_problem_set_groups.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+    lib.tb200_fetch_group_results.argtypes = [C.c_void_p, C.POINTER(GroupResults)]
     _LIB = lib
     return lib
 
@@ -272,4 +288,5 @@ EXPORTED_SYMBOLS = [
     "tb200_solve_batch", "tb200_solve_batch_resident", "tb200_fetch_results", "tb200_convexify_batch",
     "tb200_qp_solve_batch", "tb200_last_qp_polish", "tb200_last_timing",
     "tb200_qp_solve_general", "tb200_qp_general_last_error", "tb200_osqp_order_qp_settings", "tb200_problem_set_sqp_params",
+    "tb200_problem_set_groups", "tb200_fetch_group_results",
 ]

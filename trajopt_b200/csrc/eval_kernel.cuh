@@ -979,6 +979,10 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
     if (finished) {
       misc[1] = 1;
       p.status[b] = status;
+      if (status == 0 && p.group_stop) {  // release: the siblings read the flag at their next iteration top (solve_kernel.cuh)
+        __threadfence();
+        atomicExch(p.group_done + b / p.group_size, 1);
+      }
       atomicSub(p.active_count, 1);
     } else {
       misc[1] = 0;

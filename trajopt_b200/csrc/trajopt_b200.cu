@@ -6,8 +6,10 @@
 // every trajectory's QP subproblems, merit evaluations, re-convexifications and accept/shrink/penalty decisions.
 // CUDA only: every entry point fails with TB200_ERR_CUDA / TB200_ERR_NO_DEVICE when no device is usable.
 #include <cuda_runtime.h>
+#include <math_constants.h>
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -53,6 +55,19 @@ struct DevBuf {
   }
 };
 
+int checkGroups(int B, int group_size, int group_stop) {
+  if (group_size < 0) return fail(TB200_ERR_INVALID, "group_size must be >= 0 (0 or 1: no groups)");
+  if (group_size > 1 && B % group_size != 0)
+    return fail(TB200_ERR_INVALID, "batch " + std::to_string(B) + " is not a multiple of group_size " + std::to_string(group_size));
+  if (group_stop != 0 && group_stop != 1) return fail(TB200_ERR_INVALID, "group_stop must be 0 or 1");
+  return TB200_OK;
+}
+// G = 0 and G = 1 are both "no groups": every trajectory is its own group and nothing is stopped
+void setGroups(DevProblem& dp, int group_size, int group_stop) {
+  dp.group_size = std::max(group_size, 1);
+  dp.group_stop = dp.group_size > 1 ? group_stop : 0;
+}
+
 void quatToRot(const double* q, double* R) {
   double w = q[0], x = q[1], y = q[2], z = q[3];
   const double n = std::sqrt(w * w + x * x + y * y + z * z);
@@ -88,7 +103,12 @@ struct tb200_problem {
   DevBuf<double> x, new_x, trust, merit_coeffs, cost_vals, cnt_viols, new_cost_vals, new_cnt_viols, model_cost_vals,
       model_cnt_viols, cart_err, cart_jac, coll_rows, rows, ws_x, ws_yb, scratch, ws_rho, x_tmp, trust_tmp, dbg, trace, factor_g, cast_scratch, soa;
   DevBuf<unsigned long long> sched_timers, clock_start;
-  DevBuf<int> sched_state, sqp_top, time_limited, qp_paths;
+  DevBuf<int> sched_state, sqp_top, ended_by, group_done, qp_paths;
+  // the best seed of every group (group_select_kernel): [NG] index, status, n_converged, total cost; [NG][N] its x
+  DevBuf<int> g_best, g_status, g_n_converged;
+  DevBuf<double> g_total_cost, g_x;
+  int solved_group_size = 0;  // group_size of the last solve (0: no solve yet)
+  bool selected = false;      // g_* hold the selection of the last solve
   DevBuf<unsigned long long> coll_mask;
   DevBuf<int> status, sqp_iter, merit_round, qp_failures, qp_status, cur_buf, n_qp_solves, n_func_evals, n_admm_iters,
       active_count, row_ints, lists, ws_meta, tmp_iters, tmp_polish, trace_len, qp_done, lvs_overflow, link_chain, work_counter;
@@ -105,7 +125,7 @@ struct tb200_problem {
     x.release(); new_x.release(); trust.release(); merit_coeffs.release(); cost_vals.release(); cnt_viols.release();
     new_cost_vals.release(); new_cnt_viols.release(); model_cost_vals.release(); model_cnt_viols.release();
     cart_err.release(); cart_jac.release(); coll_rows.release(); rows.release(); ws_x.release(); ws_yb.release();
-    scratch.release(); ws_rho.release(); dbg.release(); trace.release(); trace_len.release(); factor_g.release(); cast_scratch.release(); soa.release(); lvs_overflow.release(); link_chain.release(); work_counter.release(); qp_done.release(); sched_state.release(); sched_timers.release(); clock_start.release(); sqp_top.release(); time_limited.release(); qp_paths.release(); x_tmp.release(); trust_tmp.release(); coll_mask.release(); status.release();
+    scratch.release(); ws_rho.release(); dbg.release(); trace.release(); trace_len.release(); factor_g.release(); cast_scratch.release(); soa.release(); lvs_overflow.release(); link_chain.release(); work_counter.release(); qp_done.release(); sched_state.release(); sched_timers.release(); clock_start.release(); sqp_top.release(); ended_by.release(); group_done.release(); qp_paths.release(); g_best.release(); g_status.release(); g_n_converged.release(); g_total_cost.release(); g_x.release(); x_tmp.release(); trust_tmp.release(); coll_mask.release(); status.release();
     sqp_iter.release(); merit_round.release(); qp_failures.release(); qp_status.release(); cur_buf.release();
     n_qp_solves.release(); n_func_evals.release(); n_admm_iters.release(); active_count.release(); row_ints.release();
     lists.release(); ws_meta.release(); tmp_iters.release(); tmp_polish.release();
@@ -114,7 +134,7 @@ struct tb200_problem {
 
 extern "C" {
 
-const char* tb200_version(void) { return "trajopt_b200 0.2 (sm_90a)"; }
+const char* tb200_version(void) { return "trajopt_b200 0.3 (sm_90a)"; }
 const char* tb200_last_error(void) { return g_err.c_str(); }
 
 void tb200_default_sqp_params(tb200_sqp_params* p) {  // optimizers.hpp:92-135
@@ -165,6 +185,7 @@ int tb200_problem_create(const tb200_problem_desc* d, int device, tb200_problem*
   if (T < 1 || T > TB200_MAX_STEPS) return fail(TB200_ERR_INVALID, "n_steps out of range");
   if (D < 1 || D > TB200_MAX_DOF) return fail(TB200_ERR_INVALID, "n_dof out of range");
   if (B < 1) return fail(TB200_ERR_INVALID, "batch must be >= 1");
+  if (int rc = checkGroups(B, d->group_size, d->group_stop)) return rc;
   if (d->robot.n_segments < 1 || d->robot.n_segments > kMaxSeg) return fail(TB200_ERR_INVALID, "n_segments out of range");
   if (d->robot.n_spheres > kMaxSpheres) return fail(TB200_ERR_INVALID, "too many collision spheres");
   if (!d->init_traj) return fail(TB200_ERR_INVALID, "init_traj is required");
@@ -618,7 +639,8 @@ int tb200_problem_create(const tb200_problem_desc* d, int device, tb200_problem*
   ALLOC(cur_buf, Bs); ALLOC(n_qp_solves, Bs); ALLOC(n_func_evals, Bs); ALLOC(n_admm_iters, Bs); ALLOC(active_count, 2);
   ALLOC(dbg, Bs * 16);
   ALLOC(sched_state, Bs); ALLOC(sched_timers, 8 + 2 * Bs);
-  ALLOC(clock_start, 1); ALLOC(sqp_top, Bs); ALLOC(time_limited, Bs);
+  ALLOC(clock_start, 1); ALLOC(sqp_top, Bs); ALLOC(ended_by, Bs); ALLOC(group_done, Bs);
+  ALLOC(g_best, Bs); ALLOC(g_status, Bs); ALLOC(g_n_converged, Bs); ALLOC(g_total_cost, Bs); ALLOC(g_x, Bs * N);
   ALLOC(trace_len, Bs);
   ALLOC(x_tmp, Bs * N); ALLOC(trust_tmp, Bs); ALLOC(tmp_iters, Bs); ALLOC(tmp_polish, Bs);
 #undef ALLOC
@@ -637,7 +659,7 @@ int tb200_problem_create(const tb200_problem_desc* d, int device, tb200_problem*
   dp.rows = P->rows.p; dp.row_ints = P->row_ints.p; dp.lists = P->lists.p; dp.ws_x = P->ws_x.p; dp.ws_yb = P->ws_yb.p;
   dp.scratch = P->scratch.p; dp.ws_meta = P->ws_meta.p; dp.ws_rho = P->ws_rho.p; dp.dbg = P->dbg.p; dp.sched_state = P->sched_state.p; dp.sched_timers = P->sched_timers.p; dp.trace_len = P->trace_len.p; dp.trace = nullptr; dp.trace_cap = 0;
   dp.soa = P->soa.p;
-  dp.clock_start = P->clock_start.p; dp.sqp_top = P->sqp_top.p; dp.time_limited = P->time_limited.p;
+  dp.clock_start = P->clock_start.p; dp.sqp_top = P->sqp_top.p; dp.ended_by = P->ended_by.p; dp.group_done = P->group_done.p;
   dp.factor_g = P->factor_g.p; dp.lvs_overflow = P->lvs_overflow.p; dp.qp_done = P->qp_done.p;
   P->ex.link_chain = P->link_chain.p;
   P->ex.work_counter = P->work_counter.p;
@@ -656,6 +678,7 @@ int tb200_problem_create(const tb200_problem_desc* d, int device, tb200_problem*
                      s.trust_shrink_ratio, s.trust_expand_ratio, s.cnt_tolerance, s.max_merit_coeff_increases,
                      s.merit_coeff_increase_ratio, s.initial_merit_error_coeff, s.trust_box_size, s.max_iter,
                      s.max_qp_solver_failures, s.inflate_constraints_individually, 0, s.max_time};
+  setGroups(dp, d->group_size, d->group_stop);
   int rc = tb200_problem_set_inputs(P, d->init_traj, d->cart_targets, d->obstacles);
   if (rc != TB200_OK) return rc;
   *out = guard.release();
@@ -676,6 +699,13 @@ int tb200_problem_set_sqp_params(tb200_problem* P, const tb200_sqp_params* s) {
                         s->trust_shrink_ratio, s->trust_expand_ratio, s->cnt_tolerance, s->max_merit_coeff_increases,
                         s->merit_coeff_increase_ratio, s->initial_merit_error_coeff, s->trust_box_size, s->max_iter,
                         s->max_qp_solver_failures, s->inflate_constraints_individually, 0, s->max_time};
+  return TB200_OK;
+}
+
+int tb200_problem_set_groups(tb200_problem* P, int32_t group_size, int32_t group_stop) {
+  if (!P) return fail(TB200_ERR_INVALID, "null problem");
+  if (int rc = checkGroups(P->B, group_size, group_stop)) return rc;
+  setGroups(P->dp, group_size, group_stop);
   return TB200_OK;
 }
 
@@ -729,7 +759,92 @@ __global__ void reset_state_kernel(DevProblem p) {
   p.ws_rho[b] = p.qp.rho;
   p.trace_len[b] = 0;
   p.sqp_top[b] = 0;  // (set by the initial evaluation)
-  p.time_limited[b] = 0;
+  p.ended_by[b] = 0;
+  if (b < p.B / p.group_size) p.group_done[b] = 0;
+}
+
+struct GroupOut {
+  int *best, *status, *n_converged;
+  double *total_cost, *x;
+};
+// Selection key of one seed (tb200_group_results): not converged, its worst constraint violation when not converged, total
+// cost, index; a NaN reads as +inf.  Smaller is better.
+struct SeedKey {
+  int failed;
+  double viol, cost;
+  int index;
+};
+__device__ __forceinline__ bool key_less(const SeedKey& a, const SeedKey& b) {
+  if (a.failed != b.failed) return a.failed < b.failed;
+  if (a.viol != b.viol) return a.viol < b.viol;
+  if (a.cost != b.cost) return a.cost < b.cost;
+  return a.index < b.index;
+}
+__device__ __forceinline__ double nan_as_inf(double v) { return v != v ? CUDART_INF : v; }
+// total_cost as tb200_fetch_results sums it (results_.total_cost = vecSum(cost_vals)): the same bits
+__device__ __forceinline__ double total_cost_of(const DevProblem& p, int b) {
+  double s = 0;
+  for (int i = 0; i < p.n_costs; ++i) s += p.cost_vals[static_cast<size_t>(b) * p.n_costs + i];
+  return s;
+}
+
+// The best seed of every group from the final per-trajectory results: one warp per group, each lane keys the seeds
+// lane, lane + 32, ... of its group, a butterfly reduction leaves the minimum on every lane, and the warp copies the
+// winner's x (two doubles per load when the rows are 16-byte aligned).
+__global__ void group_select_kernel(const DevProblem p, const GroupOut g) {
+  const int lane = threadIdx.x & 31;
+  const int grp = static_cast<int>((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  const int G = p.group_size;
+  if (grp >= p.B / G) return;  // (whole warps)
+  SeedKey best{2, CUDART_INF, CUDART_INF, INT_MAX};
+  int n_conv = 0;
+  for (int k = lane; k < G; k += 32) {
+    const int b = grp * G + k;
+    SeedKey s{p.status[b] != 0, 0.0, nan_as_inf(total_cost_of(p, b)), b};
+    if (s.failed) {
+      const double* kv = p.cnt_viols + static_cast<size_t>(b) * p.n_cnts;
+      for (int i = 0; i < p.n_cnts; ++i) s.viol = fmax(s.viol, nan_as_inf(kv[i]));
+    }
+    n_conv += !s.failed;
+    if (key_less(s, best)) best = s;
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    SeedKey other;
+    other.failed = __shfl_xor_sync(0xffffffffu, best.failed, o);
+    other.viol = __shfl_xor_sync(0xffffffffu, best.viol, o);
+    other.cost = __shfl_xor_sync(0xffffffffu, best.cost, o);
+    other.index = __shfl_xor_sync(0xffffffffu, best.index, o);
+    if (key_less(other, best)) best = other;
+    n_conv += __shfl_xor_sync(0xffffffffu, n_conv, o);
+  }
+  const int w = best.index;
+  if (lane == 0) {
+    g.best[grp] = w;
+    g.status[grp] = p.status[w];
+    g.total_cost[grp] = total_cost_of(p, w);
+    g.n_converged[grp] = n_conv;
+  }
+  const double* src = p.x + static_cast<size_t>(w) * p.N;
+  double* dst = g.x + static_cast<size_t>(grp) * p.N;
+  if ((p.N & 1) == 0) {
+    const double2* s2 = reinterpret_cast<const double2*>(src);
+    double2* d2 = reinterpret_cast<double2*>(dst);
+    for (int i = lane; i < p.N / 2; i += 32) d2[i] = s2[i];
+  } else {
+    for (int i = lane; i < p.N; i += 32) dst[i] = src[i];
+  }
+}
+
+// Launches the selection for groups of G seeds on the solver's stream.
+int launchGroupSelect(tb200_problem* P, int G) {
+  DevProblem dp = P->dp;
+  dp.group_size = G;
+  const int NG = dp.B / G;
+  const GroupOut g{P->g_best.p, P->g_status.p, P->g_n_converged.p, P->g_total_cost.p, P->g_x.p};
+  group_select_kernel<<<(NG + 3) / 4, 128, 0, P->stream>>>(dp, g);
+  CK(cudaGetLastError());
+  P->selected = true;
+  return TB200_OK;
 }
 
 cudaEvent_t getEvent(tb200_problem* P, size_t i) {
@@ -767,6 +882,13 @@ int tb200_solve_batch_resident(tb200_problem* P) {
   ctl.sched_state = dp.sched_state;
   ctl.timers = dp.sched_timers;
   solve_kernel_for(P->D, P->pair_rows)<<<std::min(dp.B, P->n_sm), kQpThreads, P->solve_smem, st>>>(dp, P->ex, ctl);
+  // the best seed of every group, inside the timed region (without groups the identity selection is made only when
+  // tb200_fetch_group_results asks for it)
+  P->solved_group_size = dp.group_size;
+  P->selected = false;
+  if (dp.group_size > 1) {
+    if (int rc = launchGroupSelect(P, dp.group_size)) return rc;
+  }
   CK(cudaEventRecord(e_end, st));
   CK(cudaStreamSynchronize(st));
   CK(cudaGetLastError());
@@ -851,6 +973,27 @@ int tb200_fetch_results(tb200_problem* P, tb200_results* out) {
       out->total_cost[b] = s;
     }
   P->timing.d2h_bytes = bytes;
+  return TB200_OK;
+}
+
+int tb200_fetch_group_results(tb200_problem* P, tb200_group_results* out) {
+  if (!P || !out) return fail(TB200_ERR_INVALID, "null argument");
+  if (P->solved_group_size == 0) return fail(TB200_ERR_INVALID, "no solve yet");
+  CK(cudaSetDevice(P->device));
+  if (!P->selected) {
+    if (int rc = launchGroupSelect(P, P->solved_group_size)) return rc;
+  }
+  const size_t B = P->dp.B, NG = B / P->solved_group_size, N = P->dp.N;
+  auto pull = [&](void* dst, const void* src, size_t n) {
+    return dst ? cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, P->stream) : cudaSuccess;
+  };
+  CK(pull(out->best, P->g_best.p, NG * sizeof(int)));
+  CK(pull(out->status, P->g_status.p, NG * sizeof(int)));
+  CK(pull(out->total_cost, P->g_total_cost.p, NG * sizeof(double)));
+  CK(pull(out->x, P->g_x.p, NG * N * sizeof(double)));
+  CK(pull(out->n_converged, P->g_n_converged.p, NG * sizeof(int)));
+  CK(pull(out->ended_by, P->ended_by.p, B * sizeof(int)));
+  CK(cudaStreamSynchronize(P->stream));
   return TB200_OK;
 }
 
@@ -977,13 +1120,23 @@ int tb200_debug_schedule(tb200_problem* P, unsigned long long* out) {
 }
 
 /* not part of the public header: the time limit of the last solve: *start_ns = %globaltimer at its start (the clock
-   the limit is measured on, comparable with tb200_debug_schedule's times), ended[b] = 1 when trajectory b was ended by
-   the limit */
+   the limit is measured on, comparable with tb200_debug_schedule's times), ended[b] = what ended trajectory b:
+   1 the limit, 2 its group (group_stop), 0 its own SQP */
 int tb200_debug_time_limit(tb200_problem* P, unsigned long long* start_ns, int32_t* ended) {
   if (!P || !start_ns || !ended) return fail(TB200_ERR_INVALID, "null argument");
   CK(cudaSetDevice(P->device));
   CK(cudaMemcpy(start_ns, P->clock_start.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-  CK(cudaMemcpy(ended, P->time_limited.p, static_cast<size_t>(P->dp.B) * sizeof(int), cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(ended, P->ended_by.p, static_cast<size_t>(P->dp.B) * sizeof(int), cudaMemcpyDeviceToHost));
+  return TB200_OK;
+}
+
+/* not part of the public header: the group flags of the last solve, done[g] = 1 when a seed of group g ended
+   OPT_CONVERGED by its own SQP while group_stop was on; [batch / group_size] */
+int tb200_debug_group_done(tb200_problem* P, int32_t* done) {
+  if (!P || !done) return fail(TB200_ERR_INVALID, "null argument");
+  CK(cudaSetDevice(P->device));
+  if (P->solved_group_size == 0) return fail(TB200_ERR_INVALID, "no solve yet");
+  CK(cudaMemcpy(done, P->group_done.p, static_cast<size_t>(P->dp.B / P->solved_group_size) * sizeof(int), cudaMemcpyDeviceToHost));
   return TB200_OK;
 }
 

@@ -117,15 +117,16 @@ def config1(B=1024, T=30, seed=SEED + 1):
     return ProblemDesc(robot, T, terms, init, fixed_timesteps=[0], cart_targets=_targets_from_goal(robot, q1, robot["tool"]))
 
 
-def config2(B=1024, T=30, seed=SEED + 2, n_obstacles=8):
+def config2(B=1024, T=30, seed=SEED + 2, n_obstacles=8, obstacle_radius=0.10):
     """configs[2]: configs[1] + discrete collision CONSTRAINT (8 sphere obstacles, dist_pen 0.02, coeff 20,
-    buffer 0.01) at all non-fixed steps; per-trajectory worlds rejection-sampled for start/goal clearance 0.05."""
+    buffer 0.01) at all non-fixed steps; per-trajectory worlds rejection-sampled for start/goal clearance 0.05.
+    More and larger obstacles make the crowded world of scripts/multi_start.py."""
     robot = robots.pr2_arm("r", with_spheres=True)
     rng = np.random.default_rng(seed)
     D = 7
     q0, q1 = _sample_endpoints(rng, robot, B)
     init = interpolate(q0, q1, T)
-    obstacles = _sample_obstacles(rng, robot, q0, q1, n_obstacles)
+    obstacles = _sample_obstacles(rng, robot, q0, q1, n_obstacles, obstacle_radius)
     terms = [joint_term(TERM_JOINT_VEL, ROLE_COST, D, 0, T - 1), joint_term(TERM_JOINT_ACC, ROLE_COST, D, 0, T - 1),
              cart_pose_term(ROLE_CNT, T - 1, robot["tool"], target_slot=0),
              collision_term(ROLE_CNT, 0, T - 1, margin=0.02, coeff=20.0, buffer=0.01, fixed_steps=[0])]
@@ -133,7 +134,7 @@ def config2(B=1024, T=30, seed=SEED + 2, n_obstacles=8):
                        cart_targets=_targets_from_goal(robot, q1, robot["tool"]), obstacles=obstacles)
 
 
-def _sample_obstacles(rng, robot, q0, q1, n_obstacles):
+def _sample_obstacles(rng, robot, q0, q1, n_obstacles, radius=0.10):
     B = len(q0)
     radii = np.array([s.radius for s in robot["spheres"]])
     obstacles = np.zeros((B, n_obstacles, 4))
@@ -144,10 +145,54 @@ def _sample_obstacles(rng, robot, q0, q1, n_obstacles):
         k = 0
         while k < n_obstacles:
             c = rng.uniform(lo, hi)
-            if np.min(np.linalg.norm(ends - c, axis=1) - rr - 0.10) >= 0.05:
-                obstacles[b, k] = (*c, 0.10)
+            if np.min(np.linalg.norm(ends - c, axis=1) - rr - radius) >= 0.05:
+                obstacles[b, k] = (*c, radius)
                 k += 1
     return obstacles
+
+
+def seed_trajectories(start, goal, T, n_seeds, rng, spread, lower=None, upper=None):
+    """Initial trajectories for a multi-start solve: [P * n_seeds, T, D], the n_seeds seeds of problem p at rows
+    [p * n_seeds, (p + 1) * n_seeds) (the group layout of tb200_problem_desc.group_size).  Seed 0 is the straight joint
+    interpolation start -> goal; seed k > 0 interpolates linearly through a mid waypoint (at (T - 1) // 2) drawn
+    uniformly within +-spread of the straight line's midpoint per joint and clamped to [lower, upper].  Endpoints are
+    kept exactly.  Deterministic given the state of `rng` (numpy Generator); host-side."""
+    start = np.atleast_2d(np.asarray(start, dtype=np.float64))
+    goal = np.atleast_2d(np.asarray(goal, dtype=np.float64))
+    P, D = start.shape
+    straight = interpolate(start, goal, T)
+    out = np.repeat(straight, n_seeds, axis=0).reshape(P, n_seeds, T, D)
+    m = (T - 1) // 2
+    if n_seeds > 1 and m > 0:
+        mid = 0.5 * (start + goal)
+        off = rng.uniform(-spread, spread, size=(P, n_seeds - 1, D))
+        via = mid[:, None, :] + off
+        if lower is not None:
+            via = np.maximum(via, np.asarray(lower, dtype=np.float64))
+        if upper is not None:
+            via = np.minimum(via, np.asarray(upper, dtype=np.float64))
+        for t in range(1, T - 1):
+            if t <= m:
+                w = t / m
+                a, b = start[:, None, :], via
+            else:
+                w = (t - m) / (T - 1 - m)
+                a, b = via, goal[:, None, :]
+            out[:, 1:, t] = a * (1 - w) + b * w
+    return out.reshape(P * n_seeds, T, D)
+
+
+def with_seeds(desc, n_seeds, rng, spread, group_stop=0):
+    """The multi-start form of a description: every trajectory becomes a group of n_seeds seeds (seed_trajectories
+    between its first and last initial waypoints, clamped to the robot's limits) that share its targets and world."""
+    d = desc
+    init = seed_trajectories(d.init_traj[:, 0], d.init_traj[:, -1], d.T, n_seeds, rng, spread,
+                             d.robot_spec["lower"], d.robot_spec["upper"])
+    rep = lambda a: None if a is None else np.repeat(a, n_seeds, axis=0)  # noqa: E731
+    per_traj = bool(d.c.obstacles_per_traj)
+    return ProblemDesc(d.robot_spec, d.T, d.terms, init, fixed_timesteps=d._fixed_t, fixed_dofs=d._fixed_d,
+                       cart_targets=rep(d.cart_targets), obstacles=rep(d.obstacles) if per_traj else d.obstacles,
+                       obstacles_per_traj=per_traj, sqp=d.c.sqp, qp=d.c.qp, group_size=n_seeds, group_stop=group_stop)
 
 
 def config3(B=4096, T=50, seed=SEED + 3, n_obstacles=8, via_every=10, lvs=0.05, evaluator=COLL_LVS_CONTINUOUS):
