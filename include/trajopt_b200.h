@@ -30,7 +30,7 @@ extern "C" {
 #endif
 
 #define TB200_VERSION_MAJOR 0
-#define TB200_VERSION_MINOR 3
+#define TB200_VERSION_MINOR 4
 #define TB200_MAX_DOF 16      /* joints per manipulator group (7 single arm, 14 dual arm) */
 #define TB200_MAX_STEPS 64    /* waypoints per trajectory */
 #define TB200_MIN_CAST_ROWS_PER_PAIR 128  /* continuous collision evaluators: lower / upper limit of the active contacts */
@@ -380,6 +380,41 @@ void tb200_osqp_order_qp_settings(tb200_qp_settings* s);
 
 /* Polish outcome (1 accepted, -1 rejected, 0 not attempted) of the last tb200_qp_solve_batch call, [B]. */
 int tb200_last_qp_polish(tb200_problem* p, int32_t* polish);
+
+/* ---- trajectory collision check (tesseract's checkTrajectory; DESIGN.md section 4.6) ----------------------------
+ * Every trajectory of the batch against the problem's robot spheres and its current obstacles (as last set by
+ * tb200_problem_create or tb200_problem_set_inputs).  Every waypoint or step pair is checked: fixed steps and the
+ * margin buffer of the collision terms play no part.  A contact is a (robot sphere, obstacle) pair with signed distance
+ * < margin (0: penetration).  type is one of TB200_COLL_*, with the sub-trajectory rules of the collision terms:
+ *   DISCRETE        S = T slots, one per waypoint; sphere/sphere distance.
+ *   LVS_DISCRETE    S = T-1 slots, one per step pair; the states q0 + (q1-q0) i/n, i = 0..n, n = ceil(|q1-q0| / lvs)
+ *                   (1 when the step is no longer than lvs), both waypoints included.
+ *   CONTINUOUS      S = T-1; one swept test per pair: the capsule of each sphere centre's path between the two states
+ *                   (the chord of the true centre path) against the obstacle sphere.
+ *   LVS_CONTINUOUS  S = T-1; n swept sub-segments per pair.
+ * n has no cap.  Per slot: the minimum signed distance, the number of contacts counted over (sphere, obstacle,
+ * sub-state | sub-segment) triples, and the argmin (sphere, obstacle, sub-index) with ties to the lowest index in that
+ * order.  Spheres are numbered as in the description.  A non-finite distance counts as a contact and is reported as
+ * NaN.  Without spheres or obstacles: +inf, no contacts, argmin (-1, -1, -1). */
+typedef struct tb200_check_config {
+  int32_t type;             /* TB200_COLL_* */
+  int32_t reserved;
+  double longest_valid_segment_length; /* LVS types: > 0 */
+  double margin;            /* contact: distance < margin */
+} tb200_check_config;
+/* Caller-owned; any pointer may be NULL to skip that output.  S = T for DISCRETE, else T-1. */
+typedef struct tb200_check_results {
+  double* step_min_distance; /* [B][S] */
+  int32_t* step_contacts;    /* [B][S] */
+  int32_t* step_argmin;      /* [B][S][3] sphere, obstacle, sub-index */
+  int32_t* in_collision;     /* [B] 1: some slot has a contact */
+  int32_t* first_slot;       /* [B] first slot with a contact, -1 if none */
+  double* min_distance;      /* [B] minimum over the slots (NaN if a slot's is) */
+} tb200_check_results;
+/* x: host [B][T][D], or NULL for the x of the last solve, already on the device (tb200_solve_batch_resident -> check ->
+ * fetch needs no round trip).  TB200_ERR_INVALID for an unknown type, an LVS type with lvs <= 0 or NaN, a non-finite
+ * margin, and a NULL x before any solve. */
+int tb200_check_trajectories(tb200_problem* p, const double* x, const tb200_check_config* cfg, tb200_check_results* out);
 
 /* Timing of the last tb200_solve_batch* call, measured with CUDA events on the solver's
  * stream: total ms, convexify-kernel ms and launches, qp-kernel ms and launches. */

@@ -542,5 +542,62 @@ inline std::vector<MultiStartResult> OptimizeProblemMultiStart(TrajOptProb& prob
   return OptimizeProblemMultiStart(prob, prob.sqpParams());
 }
 
+// tesseract::collision::CollisionCheckConfig, as the reference's tests pass it to checkTrajectory: the evaluator type
+// (TB200_COLL_*), the longest valid segment length of the LVS types and the contact margin.
+struct CollisionCheckConfig {
+  int type = TB200_COLL_DISCRETE;
+  double longest_valid_segment_length = 0.005;
+  double contact_margin = 0.0;
+};
+using TrajArray = DblVec;  // one trajectory [T*D], row-major (tesseract's TrajArray is a T x D Eigen matrix)
+
+// One trajectory's collision check.  Slots: one per waypoint (DISCRETE) or per step pair (the other types).
+struct TrajectoryCheckResult {
+  bool found = false;         // some slot has a contact (distance < contact_margin)
+  int first_slot = -1;        // the first such slot
+  double min_distance = 0;    // minimum over the slots (NaN when a distance is not finite)
+  DblVec step_min_distance;   // per slot
+  IntVec step_contacts;       // per slot: (sphere, obstacle, sub-state | sub-segment) triples in contact
+};
+
+// checkTrajectory for every trajectory of the batch (tb200_check_trajectories): trajs, one TrajArray per trajectory, or
+// nullptr for the trajectories of the last solve (they stay on the device).
+inline std::vector<TrajectoryCheckResult> checkTrajectories(TrajOptProb& prob, const CollisionCheckConfig& config,
+                                                            const std::vector<TrajArray>* trajs = nullptr) {
+  const size_t B = prob.GetBatch(), T = prob.GetNumSteps(), N = T * prob.GetNumDOF();
+  DblVec x;
+  if (trajs) {
+    if (trajs->size() != B) throw std::runtime_error("checkTrajectories: one trajectory per problem of the batch is required");
+    for (const TrajArray& t : *trajs) {
+      if (t.size() != N) throw std::runtime_error("checkTrajectories: a trajectory has the wrong size");
+      x.insert(x.end(), t.begin(), t.end());
+    }
+  }
+  const size_t S = (config.type == TB200_COLL_DISCRETE) ? T : T - 1;
+  DblVec smin(B * S), mind(B);
+  std::vector<int32_t> cont(B * S), incoll(B), first(B);
+  tb200_check_config c{};
+  c.type = config.type;
+  c.longest_valid_segment_length = config.longest_valid_segment_length;
+  c.margin = config.contact_margin;
+  tb200_check_results r{};
+  r.step_min_distance = S ? smin.data() : nullptr;
+  r.step_contacts = S ? cont.data() : nullptr;
+  r.in_collision = incoll.data();
+  r.first_slot = first.data();
+  r.min_distance = mind.data();
+  if (tb200_check_trajectories(prob.handle(), trajs ? x.data() : nullptr, &c, &r) != TB200_OK)
+    throw std::runtime_error(tb200_last_error());
+  std::vector<TrajectoryCheckResult> out(B);
+  for (size_t b = 0; b < B; ++b) {
+    out[b].found = incoll[b] != 0;
+    out[b].first_slot = first[b];
+    out[b].min_distance = mind[b];
+    out[b].step_min_distance.assign(smin.begin() + b * S, smin.begin() + (b + 1) * S);
+    out[b].step_contacts.assign(cont.begin() + b * S, cont.begin() + (b + 1) * S);
+  }
+  return out;
+}
+
 }  // namespace trajopt
 }  // namespace trajopt_b200

@@ -104,6 +104,29 @@ class Problem:
         self._check(self.lib.tb200_last_timing(self.handle, C.byref(t)))
         return {k: getattr(t, k) for k, _ in capi.Timing._fields_}
 
+    def check(self, x=None, type=capi.COLL_DISCRETE, lvs=0.005, margin=0.0):
+        """Collision check of every trajectory (tesseract's checkTrajectory): x [B][T][D], or None for the x of the last
+        solve (already on the device).  type: capi.COLL_*; lvs: longest valid segment length of the LVS types; margin:
+        a contact is a (sphere, obstacle) pair closer than it.  Returns, per slot (S = T for DISCRETE, else T - 1),
+        step_min_distance [B][S], step_contacts [B][S] and step_argmin [B][S][3] (sphere, obstacle, sub-index), and per
+        trajectory in_collision [B] (bool), first_slot [B] (-1: none) and min_distance [B]."""
+        d = self.desc
+        S = d.T if type == capi.COLL_DISCRETE else max(d.T - 1, 0)
+        out = dict(step_min_distance=np.zeros((d.B, S)), step_contacts=np.zeros((d.B, S), np.int32),
+                   step_argmin=np.zeros((d.B, S, 3), np.int32), in_collision=np.zeros(d.B, np.int32),
+                   first_slot=np.zeros(d.B, np.int32), min_distance=np.zeros(d.B))
+        r = capi.CheckResults(*[(_ip if v.dtype == np.int32 else _dp)(v) if v.size else None for v in out.values()])
+        cfg = capi.CheckConfig(type, 0, lvs, margin)
+        xp = None
+        if x is not None:
+            x = np.ascontiguousarray(x, dtype=np.float64)
+            if x.shape != (d.B, d.T, d.D):
+                raise ValueError(f"x has shape {x.shape}, expected {(d.B, d.T, d.D)}")
+            xp = _dp(x)
+        self._check(self.lib.tb200_check_trajectories(self.handle, xp, C.byref(cfg), C.byref(r)))
+        out["in_collision"] = out["in_collision"].astype(bool)
+        return out
+
     def convexify(self, x):
         L, d = self.layout, self.desc
         x = np.ascontiguousarray(x, dtype=np.float64)
@@ -161,6 +184,15 @@ def solve(desc, device=0, group_size=None, group_stop=None):
         if group_size is not None:
             out["groups"] = p.group_results()
         return out
+    finally:
+        p.close()
+
+
+def check(desc, x, type=capi.COLL_DISCRETE, lvs=0.005, margin=0.0, device=0):
+    """One-shot collision check of the trajectories x [B][T][D] against desc's robot and obstacles (Problem.check)."""
+    p = Problem(desc, device)
+    try:
+        return p.check(x, type=type, lvs=lvs, margin=margin)
     finally:
         p.close()
 

@@ -108,6 +108,17 @@ class Layout(C.Structure):
                 ("n_vars", C.c_int32), ("reserved", C.c_int32)]
 
 
+class CheckConfig(C.Structure):
+    """tb200_check_config: the trajectory collision check (type COLL_*, lvs for the LVS types, contact margin)."""
+    _fields_ = [("type", C.c_int32), ("reserved", C.c_int32), ("longest_valid_segment_length", C.c_double),
+                ("margin", C.c_double)]
+
+
+class CheckResults(C.Structure):
+    _fields_ = [("step_min_distance", _dbl_p), ("step_contacts", _i32_p), ("step_argmin", _i32_p),
+                ("in_collision", _i32_p), ("first_slot", _i32_p), ("min_distance", _dbl_p)]
+
+
 class Timing(C.Structure):
     _fields_ = [("total_ms", C.c_double), ("convexify_ms", C.c_double), ("qp_ms", C.c_double),
                 ("merit_ms", C.c_double), ("convexify_launches", C.c_int32), ("qp_launches", C.c_int32),
@@ -278,6 +289,7 @@ def load_library():
     lib.tb200_default_qp_settings.argtypes = [C.POINTER(QpSettings)]
     lib.tb200_problem_set_groups.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
     lib.tb200_fetch_group_results.argtypes = [C.c_void_p, C.POINTER(GroupResults)]
+    lib.tb200_check_trajectories.argtypes = [C.c_void_p, _dbl_p, C.POINTER(CheckConfig), C.POINTER(CheckResults)]
     _LIB = lib
     return lib
 
@@ -288,5 +300,5 @@ EXPORTED_SYMBOLS = [
     "tb200_solve_batch", "tb200_solve_batch_resident", "tb200_fetch_results", "tb200_convexify_batch",
     "tb200_qp_solve_batch", "tb200_last_qp_polish", "tb200_last_timing",
     "tb200_qp_solve_general", "tb200_qp_general_last_error", "tb200_osqp_order_qp_settings", "tb200_problem_set_sqp_params",
-    "tb200_problem_set_groups", "tb200_fetch_group_results",
+    "tb200_problem_set_groups", "tb200_fetch_group_results", "tb200_check_trajectories",
 ]

@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "../../include/trajopt_b200.h"
+#include "check_kernel.cuh"
 #include "eval_kernel.cuh"
 #include "solve_kernel.cuh"
 #include "kernels.h"
@@ -109,6 +110,10 @@ struct tb200_problem {
   DevBuf<double> g_total_cost, g_x;
   int solved_group_size = 0;  // group_size of the last solve (0: no solve yet)
   bool selected = false;      // g_* hold the selection of the last solve
+  // results of tb200_check_trajectories: [B][T] per slot (minimum, contacts, argmin x3), [B] per trajectory; allocated
+  // by the first check
+  DevBuf<double> chk_slot_min, chk_min;
+  DevBuf<int> chk_slot_contacts, chk_slot_argmin, chk_in_collision, chk_first;
   DevBuf<unsigned long long> coll_mask;
   DevBuf<int> status, sqp_iter, merit_round, qp_failures, qp_status, cur_buf, n_qp_solves, n_func_evals, n_admm_iters,
       active_count, row_ints, lists, ws_meta, tmp_iters, tmp_polish, trace_len, qp_done, lvs_overflow, link_chain, work_counter;
@@ -129,12 +134,14 @@ struct tb200_problem {
     sqp_iter.release(); merit_round.release(); qp_failures.release(); qp_status.release(); cur_buf.release();
     n_qp_solves.release(); n_func_evals.release(); n_admm_iters.release(); active_count.release(); row_ints.release();
     lists.release(); ws_meta.release(); tmp_iters.release(); tmp_polish.release();
+    chk_slot_min.release(); chk_min.release(); chk_slot_contacts.release(); chk_slot_argmin.release(); chk_in_collision.release();
+    chk_first.release();
   }
 };
 
 extern "C" {
 
-const char* tb200_version(void) { return "trajopt_b200 0.3 (sm_90a)"; }
+const char* tb200_version(void) { return "trajopt_b200 0.4 (sm_90a)"; }
 const char* tb200_last_error(void) { return g_err.c_str(); }
 
 void tb200_default_sqp_params(tb200_sqp_params* p) {  // optimizers.hpp:92-135
@@ -1186,6 +1193,51 @@ int tb200_debug_last_qp(tb200_problem* P, double* out) {
   if (!P || !out) return fail(TB200_ERR_INVALID, "null argument");
   CK(cudaSetDevice(P->device));
   CK(cudaMemcpy(out, P->dbg.p, static_cast<size_t>(P->dp.B) * 16 * sizeof(double), cudaMemcpyDeviceToHost));
+  return TB200_OK;
+}
+
+int tb200_check_trajectories(tb200_problem* P, const double* x, const tb200_check_config* cfg, tb200_check_results* out) {
+  if (!P || !cfg || !out) return fail(TB200_ERR_INVALID, "null argument");
+  const int type = cfg->type;
+  if (type != TB200_COLL_DISCRETE && type != TB200_COLL_LVS_DISCRETE && type != TB200_COLL_CONTINUOUS &&
+      type != TB200_COLL_LVS_CONTINUOUS)
+    return fail(TB200_ERR_INVALID, "unknown collision check type " + std::to_string(type) +
+                                       " (1 DISCRETE, 2 LVS_DISCRETE, 3 CONTINUOUS, 4 LVS_CONTINUOUS)");
+  if ((type == TB200_COLL_LVS_DISCRETE || type == TB200_COLL_LVS_CONTINUOUS) && !(cfg->longest_valid_segment_length > 0.0))
+    return fail(TB200_ERR_INVALID, "longest_valid_segment_length must be > 0 for the LVS check types");
+  if (!std::isfinite(cfg->margin)) return fail(TB200_ERR_INVALID, "the check margin must be finite");
+  if (!x && P->solved_group_size == 0) return fail(TB200_ERR_INVALID, "x is NULL and there is no solve whose result could be checked");
+  CK(cudaSetDevice(P->device));
+  const DevProblem& dp = P->dp;
+  const size_t B = dp.B, T = dp.T;
+  if (!P->chk_min.p) {
+    CK(P->chk_slot_min.alloc(B * T)); CK(P->chk_slot_contacts.alloc(B * T)); CK(P->chk_slot_argmin.alloc(B * T * 3));
+    CK(P->chk_in_collision.alloc(B)); CK(P->chk_first.alloc(B)); CK(P->chk_min.alloc(B));
+  }
+  cudaStream_t st = P->stream;
+  if (x) CK(cudaMemcpyAsync(P->x_tmp.p, x, B * dp.N * sizeof(double), cudaMemcpyHostToDevice, st));
+  CheckArgs a{};
+  a.segs = dp.segs; a.spheres = dp.spheres; a.obstacles = dp.obstacles;
+  a.x = x ? P->x_tmp.p : dp.x;  // NULL: the iterates the last solve left on the device
+  a.B = dp.B; a.T = dp.T; a.D = dp.D; a.S = dp.S; a.L = dp.L; a.O = dp.O; a.obstacles_per_traj = dp.obstacles_per_traj;
+  a.type = type;
+  a.n_slots = (type == TB200_COLL_DISCRETE) ? dp.T : dp.T - 1;
+  a.lvs = cfg->longest_valid_segment_length;
+  a.margin = cfg->margin;
+  a.slot_min = P->chk_slot_min.p; a.slot_contacts = P->chk_slot_contacts.p; a.slot_argmin = P->chk_slot_argmin.p;
+  a.in_collision = P->chk_in_collision.p; a.first_slot = P->chk_first.p; a.min_distance = P->chk_min.p;
+  CK(launch_check_trajectories(a, P->n_sm, st));
+  const size_t S = a.n_slots;
+  auto pull = [&](void* dst, const void* src, size_t n) {
+    return (dst && n) ? cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToHost, st) : cudaSuccess;
+  };
+  CK(pull(out->step_min_distance, a.slot_min, B * S * sizeof(double)));
+  CK(pull(out->step_contacts, a.slot_contacts, B * S * sizeof(int)));
+  CK(pull(out->step_argmin, a.slot_argmin, B * S * 3 * sizeof(int)));
+  CK(pull(out->in_collision, a.in_collision, B * sizeof(int)));
+  CK(pull(out->first_slot, a.first_slot, B * sizeof(int)));
+  CK(pull(out->min_distance, a.min_distance, B * sizeof(double)));
+  CK(cudaStreamSynchronize(st));
   return TB200_OK;
 }
 
