@@ -1,6 +1,6 @@
 #!/bin/bash
 # Builds trajopt_b200/csrc/libtb200_alt.so: the product library with the 7-joint SQP kernel compiled with extra
-# defines (kernel experiments: TB200_LIB=<path> selects it).  usage: scripts/build_alt.sh -DTB200_HYB_F0_REGS
+# defines (kernel experiments: TB200_LIB=<path> selects it).  usage: scripts/build_alt.sh -DTB200_PROFILE
 set -e
 cd "$(dirname "$0")/../trajopt_b200/csrc"
 FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -ccbin /usr/bin/g++"

@@ -572,12 +572,10 @@ __device__ inline void bcr_solve(const QpCtx& q, double* v, double* w) {
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Register-resident variant of the solve for the ADMM loop.  The factor does not change between two
-// refactorisations, and every thread applies the same few matrix rows in every solve: level 0 gives each
-// thread one forward row (NB doubles) and one backward row (NB + NB/2), and the upper levels are spread over
-// the threads so that nobody owns more than one upper forward and one upper backward row.  A solve then
-// reads only the right-hand side from shared memory (16-byte broadcasts): per level ~NB loads instead of
-// ~3*NB, no bank conflicts, and a third of the instructions.
+// Fixed per-thread roles in the solve (bcr_solve_hyb, bcr_solve_sm), computed once per block.  The factor does not
+// change between two refactorisations, and every thread applies the same few matrix rows in every solve: level 0 gives
+// each thread one forward row (NB doubles) and one backward row (NB + NB/2), and the upper levels are spread over
+// the threads so that nobody owns more than one upper forward and one upper backward row.
 struct SolveRoles {
   int n_fwd, n_lvl;                       // forward levels, all levels (the last ones only go up)
   int f0_warps, b0_warps;                 // thread ranges (rounded up to warps) with level-0 work
@@ -663,20 +661,7 @@ __host__ __device__ inline bool solve_roles_fit(int M, int NB) {
   for (int l = 1; (1 << l) - 1 < M; ++l) b += 2 * ((M + (1 << l)) >> (l + 1)) * NB;
   return f <= kQpThreads && b <= kQpThreads && 2 * ((M + 1) >> 1) * NB <= kQpThreads;
 }
-// the thread's matrix rows, from the factor in shared memory
-template <int NB>
-__device__ __forceinline__ void load_fwd_row(const QpCtx& q, int l, int u, double (&m)[NB]) {
-  constexpr int BLK = NB * NB;
-  const int M = q.M, s = 1 << l, sh = l + 1, nS = M >> sh;
-  const int task = u >> 1, side = u & 1, e = task / NB, r = task % NB;
-  const bool act = e < nS;
-  const int j = 2 * s - 1 + ((act ? e : 0) << sh);
-  const int pb = side ? j + s : j - s;
-  const bool valid = act && pb < M;
-  const double* row = (side ? q.SLM : q.SU) + (valid ? pb : j - s) * BLK + r * NB;
-#pragma unroll
-  for (int k = 0; k < NB; ++k) m[k] = valid ? row[k] : 0.0;
-}
+// the thread's backward matrix row, from the factor in shared memory
 template <int NB>
 __device__ __forceinline__ void load_bwd_row(const QpCtx& q, int l, int u, double (&m)[NB + NB / 2]) {
   constexpr int BLK = NB * NB, H = NB / 2;
@@ -690,78 +675,6 @@ __device__ __forceinline__ void load_bwd_row(const QpCtx& q, int l, int u, doubl
   for (int k = 0; k < NB; ++k) m[k] = act ? X[k * NB] : 0.0;
 #pragma unroll
   for (int k = 0; k < H; ++k) m[NB + k] = act ? Um[k * NB] : 0.0;
-}
-template <int NB>
-__device__ __forceinline__ double fwd_dot(const double (&m)[NB], const double* y) {
-  const double2* y2 = reinterpret_cast<const double2*>(y);
-  double a0 = 0.0, a1 = 0.0;
-#pragma unroll
-  for (int k = 0; k < NB / 2; ++k) {
-    const double2 yy = y2[k];
-    a0 += m[2 * k] * yy.x;
-    a1 += m[2 * k + 1] * yy.y;
-  }
-  return a0 + a1;
-}
-template <int NB>
-__device__ __forceinline__ double bwd_dot(const double (&m)[NB + NB / 2], const double* y, const double* wl, bool side,
-                                          bool hasl, bool hasr) {
-  const double2* y2 = reinterpret_cast<const double2*>(y);
-  double a0 = 0.0, a1 = 0.0, a2 = 0.0;
-#pragma unroll
-  for (int k = 0; k < NB / 2; ++k) {
-    const double2 yy = y2[k];
-    a0 += m[2 * k] * yy.x;
-    a1 += m[2 * k + 1] * yy.y;
-  }
-#pragma unroll
-  for (int k = 0; k < NB / 2; ++k) a2 += m[NB + k] * wl[k];
-  const double dx = a0 + a1;
-  return (side ? (hasr ? -dx : 0.0) : dx) - (hasl ? a2 : 0.0);
-}
-template <int NB>
-__device__ __forceinline__ void bcr_solve_reg(const QpCtx& q, const SolveRoles& R, const double (&mF0)[NB],
-                                              const double (&mB0)[NB + NB / 2], const double (&mFU)[NB],
-                                              const double (&mBU)[NB + NB / 2], double* v, double* w) {
-  const int tid = q.tid, wbase = tid & ~31;
-  const bool side = tid & 1;
-  __syncthreads();
-  // ---- down
-  if (wbase < R.f0_warps) {
-    double a = fwd_dot<NB>(mF0, v + R.f0_vec);
-    a = R.f0_valid ? a : 0.0;
-    const double o = __shfl_xor_sync(0xffffffffu, a, 1);
-    if (R.f0_store) v[R.f0_dst] -= a + o;
-  }
-  __syncthreads();
-  for (int l = 1; l < R.n_fwd; ++l) {
-    const bool mine = R.fu_level == l;
-    if (__any_sync(0xffffffffu, mine)) {
-      double a = fwd_dot<NB>(mFU, v + (mine ? R.fu_vec : 0));
-      a = (mine && R.fu_valid) ? a : 0.0;
-      const double o = __shfl_xor_sync(0xffffffffu, a, 1);
-      if (mine && R.fu_store) v[R.fu_dst] -= a + o;
-    }
-    __syncthreads();
-  }
-  // ---- up
-  for (int l = R.n_lvl - 1; l >= 1; --l) {
-    const bool mine = R.bu_level == l;
-    if (__any_sync(0xffffffffu, mine)) {
-      const double* y = (R.bu_yw ? w : v) + (mine ? R.bu_y : 0);
-      double acc = bwd_dot<NB>(mBU, y, w + (mine ? R.bu_wl : 0), R.bu_yw, R.bu_hasl, R.bu_hasr);
-      acc = mine ? acc : 0.0;
-      const double o = __shfl_xor_sync(0xffffffffu, acc, 1);
-      if (mine && R.bu_store) w[R.bu_dst] = acc + o;
-    }
-    __syncthreads();
-  }
-  if (wbase < R.b0_warps) {
-    const double acc = bwd_dot<NB>(mB0, (side ? w : v) + R.b0_y, w + R.b0_wl, side, R.b0_hasl, R.b0_hasr);
-    const double o = __shfl_xor_sync(0xffffffffu, acc, 1);
-    if (R.b0_store) w[R.b0_dst] = acc + o;
-  }
-  __syncthreads();
 }
 
 // Shared-memory loads that stay where they are written: every level of the solve is a short dependent chain (loads ->
@@ -887,26 +800,11 @@ __device__ __forceinline__ void bcr_solve_sm(const int tid, const SolveRoles& R,
   __syncthreads();
 }
 
-// Register-resident solve for the ADMM block (called with the whole register file at its disposal): every thread
-// applies the same few factor rows in every solve, so they live in registers (level 0: one forward and one backward
-// row; upper levels: one each for the threads that have a role there) and a level only reads the right-hand side —
+// A backward task with its factor row in registers (called with the whole register file at its disposal): every thread
+// applies the same row in every solve, so it is loaded once per block and the task only reads the right-hand side —
 // a few distinct 16-byte words per warp — from shared memory.  With the rows read from shared memory instead, level 0
 // alone would move 44 KB (down) and 75 KB (up) per solve through the 128 B/clock shared-memory port, 210 KB per solve
-// in all = 1640 cycles of pure bandwidth.  The loads of a level are issued before its multiply-adds.
-template <int NB>
-__device__ __forceinline__ double reg_fwd_task(const double (&m)[NB], const double* yv) {
-  constexpr int H = NB / 2;
-  double2 yy[H];
-#pragma unroll
-  for (int k = 0; k < H; ++k) yy[k] = lds_v2(yv + 2 * k);
-  double a0 = 0.0, a1 = 0.0;
-#pragma unroll
-  for (int k = 0; k < H; ++k) {
-    a0 += m[2 * k] * yy[k].x;
-    a1 += m[2 * k + 1] * yy[k].y;
-  }
-  return a0 + a1;
-}
+// in all = 1640 cycles of pure bandwidth.  The loads are issued before the multiply-adds.
 template <int NB>
 __device__ __forceinline__ double reg_bwd_task(const double (&m)[NB + NB / 2], const double* y, const double* wl, bool side,
                                                bool hasl, bool hasr) {
@@ -928,68 +826,20 @@ __device__ __forceinline__ double reg_bwd_task(const double (&m)[NB + NB / 2], c
   const double dx = a0 + a1;
   return (side ? (hasr ? -dx : 0.0) : dx) - (hasl ? a2 : 0.0);
 }
-template <int NB>
-__device__ __forceinline__ void bcr_solve_regs(const int tid, const SolveRoles& R, const double (&mF0)[NB],
-                                               const double (&mB0)[NB + NB / 2], const double (&mFU)[NB],
-                                               const double (&mBU)[NB + NB / 2], double* v, double* w) {
-  const int wbase = tid & ~31;
-  const bool side = tid & 1;
-  __syncthreads();
-  // ---- down
-  if (wbase < R.f0_warps) {
-    double a = reg_fwd_task<NB>(mF0, v + R.f0_vec);
-    a = R.f0_valid ? a : 0.0;
-    const double o = __shfl_xor_sync(0xffffffffu, a, 1);
-    if (R.f0_store) v[R.f0_dst] -= a + o;
-  }
-  __syncthreads();
-  for (int l = 1; l < R.n_fwd; ++l) {
-    const bool mine = R.fu_level == l;
-    if (__any_sync(0xffffffffu, mine)) {
-      double a = reg_fwd_task<NB>(mFU, v + (mine ? R.fu_vec : 0));
-      a = (mine && R.fu_valid) ? a : 0.0;
-      const double o = __shfl_xor_sync(0xffffffffu, a, 1);
-      if (mine && R.fu_store) v[R.fu_dst] -= a + o;
-    }
-    __syncthreads();
-  }
-  // ---- up
-  for (int l = R.n_lvl - 1; l >= 1; --l) {
-    const bool mine = R.bu_level == l;
-    if (__any_sync(0xffffffffu, mine)) {
-      double acc = reg_bwd_task<NB>(mBU, (R.bu_yw ? w : v) + (mine ? R.bu_y : 0), w + (mine ? R.bu_wl : 0), R.bu_yw,
-                                    R.bu_hasl, R.bu_hasr);
-      acc = mine ? acc : 0.0;
-      const double o = __shfl_xor_sync(0xffffffffu, acc, 1);
-      if (mine && R.bu_store) w[R.bu_dst] = acc + o;
-    }
-    __syncthreads();
-  }
-  if (wbase < R.b0_warps) {
-    const double acc = reg_bwd_task<NB>(mB0, (side ? w : v) + R.b0_y, w + R.b0_wl, side, R.b0_hasl, R.b0_hasr);
-    const double o = __shfl_xor_sync(0xffffffffu, acc, 1);
-    if (R.b0_store) w[R.b0_dst] = acc + o;
-  }
-  __syncthreads();
-}
 
-// The solve of the ADMM block: level 0 (every thread has a role there: 44 KB + 75 KB of factor rows per solve if they
-// were read from shared memory) applies rows held in registers; the upper levels (a few warps each, 91 KB per solve in
-// all) read theirs from shared memory.  All four row sets in registers (140 registers) do not fit beside the loop's own
-// state even with the whole register file.
+// The solve of admm_block_fast: the level-0 backward rows (every thread has one: 75 KB of factor rows per solve if they
+// were read from shared memory) are held in registers; the level-0 forward rows and the upper levels (a few warps each,
+// 91 KB per solve in all) are read from shared memory.  All four row sets in registers (140 registers) do not fit beside
+// the loop's own state even with the whole register file.
 template <int NB>
-__device__ __forceinline__ void bcr_solve_hyb(const int tid, const SolveRoles& R, const double (&mF0)[NB],
-                                              const double (&mB0)[NB + NB / 2], const double* sm_base, double* v, double* w) {
+__device__ __forceinline__ void bcr_solve_hyb(const int tid, const SolveRoles& R, const double (&mB0)[NB + NB / 2],
+                                              const double* sm_base, double* v, double* w) {
   const int wbase = tid & ~31;
   const bool side = tid & 1;
   __syncthreads();
   // ---- down
   if (wbase < R.f0_warps) {
-#ifndef TB200_HYB_F0_REGS  // (default: the level-0 forward rows come from shared memory, only the backward rows are register resident)
     double a = bcr_fwd_task<NB>(sm_base + R.f0_mat, v + R.f0_vec);
-#else
-    double a = reg_fwd_task<NB>(mF0, v + R.f0_vec);
-#endif
     a = R.f0_valid ? a : 0.0;
     const double o = __shfl_xor_sync(0xffffffffu, a, 1);
     if (R.f0_store) v[R.f0_dst] -= a + o;
@@ -1590,61 +1440,95 @@ __device__ __forceinline__ void row_backsub(const double* F, double zeta, double
 __device__ __forceinline__ double row_reduce_coef(const double* F, double ra0, double ra1, double zcoef) {
   return zcoef - F[R_WRR] * (F[R_U0] * ra0 * F[R_G1] + F[R_U1] * ra1 * F[R_G0]) * F[R_IDEN];
 }
+// The row work of the ADMM blocks whose rows are records (R, F, I): admm_block passes q.R(r), q.F(r), q.I(r), the
+// others their shared-memory offsets.  The scalars are references so that admm_block, which passes the fields of its
+// context, reads them where they are used (copies held across the row's stores cost it spills); the others pass
+// locals.  Entry pass: the aux right-hand sides R_RA0/1, the row multiplier R_COEF and the row's contributions to the
+// right-hand side of the next solve, from the current row state.
+template <int CNc>
+__device__ __forceinline__ void admm_row_entry(const double* R, double* F, const double& sigma, const double& rho_aux) {
+  const double s = F[R_WRR] * F[R_Z] - F[R_Y];
+  const double ra0 = sigma * F[R_XA0] - F[R_QA0] + F[R_U0] * s + F[R_B0] * (rho_aux * F[R_ZA0] - F[R_YA0]);
+  const double ra1 = sigma * F[R_XA1] - F[R_QA1] + F[R_U1] * s + F[R_B1] * (rho_aux * F[R_ZA1] - F[R_YA1]);
+  F[R_RA0] = ra0;
+  F[R_RA1] = ra1;
+  const double cf = row_reduce_coef(F, ra0, ra1, s);
+  F[R_COEF] = cf;
+#pragma unroll
+  for (int k = 0; k < CNc; ++k) F[R_NF + k] = R[CNc + k] * cf;
+}
+// After a solve w: back-substitute aux, relax, project, dual update, and the multipliers for the next solve
+// (oma = 1 - alpha, inv_rho_aux = 1 / rho_aux).
+template <int CNc>
+__device__ __forceinline__ void admm_row_update(const double* R, double* F, const int* I, const double* w,
+                                                const double& sigma, const double& alpha, const double& oma,
+                                                const double& rho_aux, const double& inv_rho_aux) {
+  double zeta = 0.0;
+  {
+    const int base = I[RI_BASE], stride = I[RI_STRIDE], last = I[RI_CNT] - 1;
+#pragma unroll
+    for (int k = 0; k < CNc; ++k) zeta += R[CNc + k] * w[base + min(k, last) * stride];
+  }
+  double a0, a1;
+  row_backsub(F, zeta, a0, a1);
+  const double zt = zeta + F[R_U0] * a0 + F[R_U1] * a1;
+  const double Wr = F[R_WRR];
+  const double zr = alpha * zt + oma * F[R_Z];
+  double zn = zr + F[R_Y] * F[R_IWRR];
+  zn = fmin(fmax(zn, F[R_LO]), F[R_UP]);
+  const double dy = Wr * (zr - zn);
+  const double yn = F[R_Y] + dy;
+  F[R_Z] = zn;
+  F[R_Y] = yn;
+  F[R_DY] = dy;
+  const double s = Wr * zn - yn;
+  double ra[2];
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    const double at = k ? a1 : a0, bb = F[R_B0 + k];
+    const double xo = F[R_XA0 + k];
+    const double xn = alpha * at + oma * xo;
+    const double zra = alpha * (bb * at) + oma * F[R_ZA0 + k];
+    double z2 = zra + F[R_YA0 + k] * inv_rho_aux;
+    z2 = fmin(fmax(z2, 0.0), kOsqpInf * F[R_EA0 + k]);
+    const double dya = rho_aux * (zra - z2);
+    const double yan = F[R_YA0 + k] + dya;
+    F[R_XA0 + k] = xn;
+    F[R_DXA0 + k] = xn - xo;
+    F[R_ZA0 + k] = z2;
+    F[R_YA0 + k] = yan;
+    F[R_DYA0 + k] = dya;
+    ra[k] = sigma * xn - F[R_QA0 + k] + F[R_U0 + k] * s + bb * (rho_aux * z2 - yan);
+  }
+  F[R_RA0] = ra[0];
+  F[R_RA1] = ra[1];
+  const double cf = row_reduce_coef(F, ra[0], ra[1], s);
+  F[R_COEF] = cf;
+#pragma unroll
+  for (int k = 0; k < CNc; ++k) F[R_NF + k] = R[CNc + k] * cf;
+}
 
 // ---------------------------------------------------------------------------------------------------
 // A block of ADMM iterations (no termination test inside): its own function (not inlined), so that the loop the
 // whole batch time hangs on has its own register allocation and sits in one contiguous piece of code — the rest of
 // the solver (scaling, residuals, certificates, polish, factorisation) cannot spill into it or push it out of the
-// instruction cache.  REG: the thread's rows of the factor live in registers for the whole block (reloaded from the
-// factor in shared memory at entry: ~100 loads per 25 iterations); else the generic solve reads them from memory.
-// Rows are handled by the high thread ids so that they run beside the per-variable work of the low ones.  Every
-// iteration leaves the aux right-hand sides R_RA0/1, the row multiplier R_COEF and the rows' contributions to the
-// right-hand side of the next solve behind; the entry pass (re)builds them because the residual passes, the polish
-// and a refactorisation reuse those fields.  keep_last: the last iteration records its primal / dual steps (dxs, dyb)
-// for the infeasibility certificates.
-template <int NB, int PAIR, bool REG>
+// instruction cache.  The generic solve reads the factor rows from memory.  Rows are handled by the high thread ids
+// so that they run beside the per-variable work of the low ones.  Every iteration leaves the aux right-hand sides
+// R_RA0/1, the row multiplier R_COEF and the rows' contributions to the right-hand side of the next solve behind; the
+// entry pass (re)builds them because the residual passes, the polish and a refactorisation reuse those fields.
+// keep_last: the last iteration records its primal / dual steps (dxs, dyb) for the infeasibility certificates.
+template <int NB, int PAIR>
 __device__ __noinline__ void admm_block(const QpCtx& q, const double rho_aux, const int n_iter, const int keep_last) {
   constexpr int CNc = PAIR ? ((NB > 3) ? NB : 3) : ((NB / 2 > 3) ? NB / 2 : 3);
-  constexpr int RNB = REG ? NB : 2;
   const int N = q.N, tid = q.tid;
   double* const dxs = q.scratch;
   double* const dyb = q.scratch + q.Np;
-  SolveRoles roles{};
-  double mF0[RNB], mB0[RNB + RNB / 2], mFU[RNB], mBU[RNB + RNB / 2];
-  if constexpr (REG) {
-    roles = solve_roles<NB>(q);
-    load_fwd_row<NB>(q, 0, tid, mF0);
-    load_bwd_row<NB>(q, 0, tid, mB0);
-    int off = 0;
-    for (int l = 1; l < roles.n_fwd; ++l) {
-      const int cnt = 2 * (q.M >> (l + 1)) * NB;
-      if (roles.fu_level == l) load_fwd_row<NB>(q, l, tid - off, mFU);
-      off += cnt;
-    }
-    off = 0;
-    for (int l = 1; l < roles.n_lvl; ++l) {
-      const int cnt = 2 * ((q.M + (1 << l)) >> (l + 1)) * NB;
-      if (roles.bu_level == l) load_bwd_row<NB>(q, l, tid - off, mBU);
-      off += cnt;
-    }
-  }
-  const bool one_var = REG || q.Np <= kQpThreads;  // one thread per variable: its column range is loop invariant
+  const bool one_var = q.Np <= kQpThreads;  // one thread per variable: its column range is loop invariant
   const int my_e0 = (one_var && tid < N) ? q.colptr[tid] : 0, my_e1 = (one_var && tid < N) ? q.colptr[tid + 1] : 0;
   {  // entry pass: aux right-hand sides, row multipliers and contributions from the current row state
     PROF_T0();
-    for (int r = kQpThreads - 1 - tid; r < q.nrows; r += kQpThreads) {
-      double* F = q.F(r);
-      const double s = F[R_WRR] * F[R_Z] - F[R_Y];
-      const double ra0 = q.sigma * F[R_XA0] - F[R_QA0] + F[R_U0] * s + F[R_B0] * (rho_aux * F[R_ZA0] - F[R_YA0]);
-      const double ra1 = q.sigma * F[R_XA1] - F[R_QA1] + F[R_U1] * s + F[R_B1] * (rho_aux * F[R_ZA1] - F[R_YA1]);
-      F[R_RA0] = ra0;
-      F[R_RA1] = ra1;
-      const double cf = row_reduce_coef(F, ra0, ra1, s);
-      F[R_COEF] = cf;
-      const double* as = q.R(r) + CNc;
-#pragma unroll
-      for (int k = 0; k < CNc; ++k) F[R_NF + k] = as[k] * cf;
-    }
+    for (int r = kQpThreads - 1 - tid; r < q.nrows; r += kQpThreads)
+      admm_row_entry<CNc>(q.R(r), q.F(r), q.sigma, rho_aux);
     __syncthreads();
     PROF_ADD(0);
   }
@@ -1685,54 +1569,13 @@ __device__ __noinline__ void admm_block(const QpCtx& q, const double rho_aux, co
     }
     {
       PROF_T0();
-      if constexpr (REG) bcr_solve_reg<NB>(q, roles, mF0, mB0, mFU, mBU, q.v1, q.w);
-      else bcr_solve<NB>(q, q.v1, q.w);
+      bcr_solve<NB>(q, q.v1, q.w);
       PROF_ADD(2);
     }
     PROF_T0();
     // rows: back-substitute aux, relax, project, dual update, and the multipliers for the next solve
-    for (int r = kQpThreads - 1 - tid; r < q.nrows; r += kQpThreads) {
-      const double* R = q.R(r);
-      double* F = q.F(r);
-      const double zeta = row_dot<CNc>(q, R, q.I(r), q.w);
-      double a0, a1;
-      row_backsub(F, zeta, a0, a1);
-      const double zt = zeta + F[R_U0] * a0 + F[R_U1] * a1;
-      const double Wr = F[R_WRR];
-      const double zr = q.alpha * zt + (1.0 - q.alpha) * F[R_Z];
-      double zn = zr + F[R_Y] * F[R_IWRR];
-      zn = fmin(fmax(zn, F[R_LO]), F[R_UP]);
-      const double dy = Wr * (zr - zn);
-      const double yn = F[R_Y] + dy;
-      F[R_Z] = zn;
-      F[R_Y] = yn;
-      F[R_DY] = dy;
-      const double s = Wr * zn - yn;
-      double ra[2];
-#pragma unroll
-      for (int k = 0; k < 2; ++k) {
-        const double at = k ? a1 : a0, bb = F[R_B0 + k];
-        const double xo = F[R_XA0 + k];
-        const double xn = q.alpha * at + (1.0 - q.alpha) * xo;
-        const double zra = q.alpha * (bb * at) + (1.0 - q.alpha) * F[R_ZA0 + k];
-        double z2 = zra + F[R_YA0 + k] * inv_rho_aux;
-        z2 = fmin(fmax(z2, 0.0), kOsqpInf * F[R_EA0 + k]);
-        const double dya = rho_aux * (zra - z2);
-        const double yan = F[R_YA0 + k] + dya;
-        F[R_XA0 + k] = xn;
-        F[R_DXA0 + k] = xn - xo;
-        F[R_ZA0 + k] = z2;
-        F[R_YA0 + k] = yan;
-        F[R_DYA0 + k] = dya;
-        ra[k] = q.sigma * xn - F[R_QA0 + k] + F[R_U0 + k] * s + bb * (rho_aux * z2 - yan);
-      }
-      F[R_RA0] = ra[0];
-      F[R_RA1] = ra[1];
-      const double cf = row_reduce_coef(F, ra[0], ra[1], s);
-      F[R_COEF] = cf;
-#pragma unroll
-      for (int k = 0; k < CNc; ++k) F[R_NF + k] = R[CNc + k] * cf;
-    }
+    for (int r = kQpThreads - 1 - tid; r < q.nrows; r += kQpThreads)
+      admm_row_update<CNc>(q.R(r), q.F(r), q.I(r), q.w, q.sigma, q.alpha, 1.0 - q.alpha, rho_aux, inv_rho_aux);
     // trajectory variables and their bound rows (one thread per variable)
     for (int i = tid; i < N; i += kQpThreads) {
       const double beta = q.beta[i];
@@ -1758,7 +1601,7 @@ __device__ __noinline__ void admm_block(const QpCtx& q, const double rho_aux, co
   }
 }
 
-// The same block of iterations for the common case — factor rows in registers (REG roles fit), QP rows in shared
+// The same block of iterations for the common case — the solve's thread roles fit the CTA, QP rows in shared
 // memory — written for the latency of ONE iteration:
 //  * every operand address is an offset into the CTA's dynamic shared memory (LDS / STS, not generic loads), every
 //    solver scalar a register (the QpCtx behind `q` is only read at entry);
@@ -1767,7 +1610,8 @@ __device__ __noinline__ void admm_block(const QpCtx& q, const double rho_aux, co
 //    rows' contributions, which are fetched through entry addresses preloaded once per block (8 per variable, the
 //    common case; longer columns walk the rest of their list);
 //  * nothing loop invariant is recomputed inside the loop.
-// The arithmetic (operations and their order) is that of admm_block.
+// The row work is admm_block's (admm_row_entry, admm_row_update); the variable's update keeps its operations and
+// their order.
 template <int NB, int PAIR>
 __device__ __noinline__ void admm_block_fast(const QpCtx& q, const double rho_aux_in, const int n_iter, const int keep_last) {
   constexpr int CNc = PAIR ? ((NB > 3) ? NB : 3) : ((NB / 2 > 3) ? NB / 2 : 3);
@@ -1784,8 +1628,7 @@ __device__ __noinline__ void admm_block_fast(const QpCtx& q, const double rho_au
   double* const dxs = q.scratch;
   double* const dyb = q.scratch + Np;
   const SolveRoles roles = solve_roles<NB>(q);
-  double mF0[NB], mB0[NB + NB / 2];  // the thread's level-0 rows of the factor
-  load_fwd_row<NB>(q, 0, tid, mF0);
+  double mB0[NB + NB / 2];  // the thread's level-0 backward row of the factor
   load_bwd_row<NB>(q, 0, tid, mB0);
   // ---- this thread's variable
   const bool has_var = tid < N;
@@ -1810,19 +1653,8 @@ __device__ __noinline__ void admm_block_fast(const QpCtx& q, const double rho_au
   // ---- this thread's row (rows are handled by the high thread ids so that they run beside the per-variable work)
   {  // entry pass: aux right-hand sides, row multipliers and contributions from the current row state
     PROF_T0();
-    for (int r = kQpThreads - 1 - tid; r < nrows; r += kQpThreads) {
-      double* F = rows + r * RS + 2 * CNc;
-      const double s = F[R_WRR] * F[R_Z] - F[R_Y];
-      const double ra0 = sigma * F[R_XA0] - F[R_QA0] + F[R_U0] * s + F[R_B0] * (rho_aux * F[R_ZA0] - F[R_YA0]);
-      const double ra1 = sigma * F[R_XA1] - F[R_QA1] + F[R_U1] * s + F[R_B1] * (rho_aux * F[R_ZA1] - F[R_YA1]);
-      F[R_RA0] = ra0;
-      F[R_RA1] = ra1;
-      const double cf = row_reduce_coef(F, ra0, ra1, s);
-      F[R_COEF] = cf;
-      const double* as = rows + r * RS + CNc;
-#pragma unroll
-      for (int k = 0; k < CNc; ++k) F[R_NF + k] = as[k] * cf;
-    }
+    for (int r = kQpThreads - 1 - tid; r < nrows; r += kQpThreads)
+      admm_row_entry<CNc>(rows + r * RS, rows + r * RS + 2 * CNc, sigma, rho_aux);
     __syncthreads();
     PROF_ADD(0);
   }
@@ -1850,59 +1682,14 @@ __device__ __noinline__ void admm_block_fast(const QpCtx& q, const double rho_au
     }
     {
       PROF_T0();
-      bcr_solve_hyb<NB>(tid, roles, mF0, mB0, sm, v1, w);
+      bcr_solve_hyb<NB>(tid, roles, mB0, sm, v1, w);
       PROF_ADD(2);
     }
     PROF_T0();
     // rows: back-substitute aux, relax, project, dual update, and the multipliers for the next solve
-    for (int r = kQpThreads - 1 - tid; r < nrows; r += kQpThreads) {
-      const double* R = rows + r * RS;
-      double* F = rows + r * RS + 2 * CNc;
-      const int* I = rints + r * RI_NINTS;
-      double zeta = 0.0;
-      {
-        const int base = I[RI_BASE], stride = I[RI_STRIDE], last = I[RI_CNT] - 1;
-#pragma unroll
-        for (int k = 0; k < CNc; ++k) zeta += R[CNc + k] * w[base + min(k, last) * stride];
-      }
-      double a0, a1;
-      row_backsub(F, zeta, a0, a1);
-      const double zt = zeta + F[R_U0] * a0 + F[R_U1] * a1;
-      const double Wr = F[R_WRR];
-      const double zr = alpha * zt + oma * F[R_Z];
-      double zn = zr + F[R_Y] * F[R_IWRR];
-      zn = fmin(fmax(zn, F[R_LO]), F[R_UP]);
-      const double dy = Wr * (zr - zn);
-      const double yn = F[R_Y] + dy;
-      F[R_Z] = zn;
-      F[R_Y] = yn;
-      F[R_DY] = dy;
-      const double s = Wr * zn - yn;
-      double ra[2];
-#pragma unroll
-      for (int k = 0; k < 2; ++k) {
-        const double at = k ? a1 : a0, bb = F[R_B0 + k];
-        const double xo = F[R_XA0 + k];
-        const double xn = alpha * at + oma * xo;
-        const double zra = alpha * (bb * at) + oma * F[R_ZA0 + k];
-        double z2 = zra + F[R_YA0 + k] * inv_rho_aux;
-        z2 = fmin(fmax(z2, 0.0), kOsqpInf * F[R_EA0 + k]);
-        const double dya = rho_aux * (zra - z2);
-        const double yan = F[R_YA0 + k] + dya;
-        F[R_XA0 + k] = xn;
-        F[R_DXA0 + k] = xn - xo;
-        F[R_ZA0 + k] = z2;
-        F[R_YA0 + k] = yan;
-        F[R_DYA0 + k] = dya;
-        ra[k] = sigma * xn - F[R_QA0 + k] + F[R_U0 + k] * s + bb * (rho_aux * z2 - yan);
-      }
-      F[R_RA0] = ra[0];
-      F[R_RA1] = ra[1];
-      const double cf = row_reduce_coef(F, ra[0], ra[1], s);
-      F[R_COEF] = cf;
-#pragma unroll
-      for (int k = 0; k < CNc; ++k) F[R_NF + k] = R[CNc + k] * cf;
-    }
+    for (int r = kQpThreads - 1 - tid; r < nrows; r += kQpThreads)
+      admm_row_update<CNc>(rows + r * RS, rows + r * RS + 2 * CNc, rints + r * RI_NINTS, w, sigma, alpha, oma, rho_aux,
+                           inv_rho_aux);
     // the thread's variable and its bound row
     if (has_var) {
       const double xt = w[vi];
@@ -2115,19 +1902,8 @@ __device__ __noinline__ void admm_block_pinv(const QpCtx& q, const double rho_au
   } else {
     // ================= warps 6-7: the QP rows, separator halves, variables
     // entry pass: aux right-hand sides, row multipliers and contributions from the current row state
-    for (int r = kQpThreads - 1 - tid; r < nrows; r += kRowThreads) {
-      double* F = rows + r * RS + 2 * CNc;
-      const double s = F[R_WRR] * F[R_Z] - F[R_Y];
-      const double ra0 = sigma * F[R_XA0] - F[R_QA0] + F[R_U0] * s + F[R_B0] * (rho_aux * F[R_ZA0] - F[R_YA0]);
-      const double ra1 = sigma * F[R_XA1] - F[R_QA1] + F[R_U1] * s + F[R_B1] * (rho_aux * F[R_ZA1] - F[R_YA1]);
-      F[R_RA0] = ra0;
-      F[R_RA1] = ra1;
-      const double cf = row_reduce_coef(F, ra0, ra1, s);
-      F[R_COEF] = cf;
-      const double* as = rows + r * RS + CNc;
-#pragma unroll
-      for (int k = 0; k < CNc; ++k) F[R_NF + k] = as[k] * cf;
-    }
+    for (int r = kQpThreads - 1 - tid; r < nrows; r += kRowThreads)
+      admm_row_entry<CNc>(rows + r * RS, rows + r * RS + 2 * CNc, sigma, rho_aux);
     bar();
     for (int it = 0; it < n_iter; ++it) {
       const bool keep_steps = keep_last && it == n_iter - 1;
@@ -2137,54 +1913,9 @@ __device__ __noinline__ void admm_block_pinv(const QpCtx& q, const double rho_au
       bar();
       bar();  // (step B of the partition warps)
       // rows: back-substitute aux, relax, project, dual update, and the multipliers for the next solve
-      for (int r = kQpThreads - 1 - tid; r < nrows; r += kRowThreads) {
-        const double* R = rows + r * RS;
-        double* F = rows + r * RS + 2 * CNc;
-        const int* I = rints + r * RI_NINTS;
-        double zeta = 0.0;
-        {
-          const int base = I[RI_BASE], stride = I[RI_STRIDE], last = I[RI_CNT] - 1;
-#pragma unroll
-          for (int k = 0; k < CNc; ++k) zeta += R[CNc + k] * w[base + min(k, last) * stride];
-        }
-        double a0, a1;
-        row_backsub(F, zeta, a0, a1);
-        const double zt = zeta + F[R_U0] * a0 + F[R_U1] * a1;
-        const double Wr = F[R_WRR];
-        const double zr = alpha * zt + oma * F[R_Z];
-        double zn = zr + F[R_Y] * F[R_IWRR];
-        zn = fmin(fmax(zn, F[R_LO]), F[R_UP]);
-        const double dy = Wr * (zr - zn);
-        const double yn = F[R_Y] + dy;
-        F[R_Z] = zn;
-        F[R_Y] = yn;
-        F[R_DY] = dy;
-        const double s = Wr * zn - yn;
-        double ra[2];
-#pragma unroll
-        for (int k = 0; k < 2; ++k) {
-          const double at = k ? a1 : a0, bb = F[R_B0 + k];
-          const double xo = F[R_XA0 + k];
-          const double xn = alpha * at + oma * xo;
-          const double zra = alpha * (bb * at) + oma * F[R_ZA0 + k];
-          double z2 = zra + F[R_YA0 + k] * inv_rho_aux;
-          z2 = fmin(fmax(z2, 0.0), kOsqpInf * F[R_EA0 + k]);
-          const double dya = rho_aux * (zra - z2);
-          const double yan = F[R_YA0 + k] + dya;
-          F[R_XA0 + k] = xn;
-          F[R_DXA0 + k] = xn - xo;
-          F[R_ZA0 + k] = z2;
-          F[R_YA0 + k] = yan;
-          F[R_DYA0 + k] = dya;
-          ra[k] = sigma * xn - F[R_QA0 + k] + F[R_U0 + k] * s + bb * (rho_aux * z2 - yan);
-        }
-        F[R_RA0] = ra[0];
-        F[R_RA1] = ra[1];
-        const double cf = row_reduce_coef(F, ra[0], ra[1], s);
-        F[R_COEF] = cf;
-#pragma unroll
-        for (int k = 0; k < CNc; ++k) F[R_NF + k] = R[CNc + k] * cf;
-      }
+      for (int r = kQpThreads - 1 - tid; r < nrows; r += kRowThreads)
+        admm_row_update<CNc>(rows + r * RS, rows + r * RS + 2 * CNc, rints + r * RI_NINTS, w, sigma, alpha, oma, rho_aux,
+                             inv_rho_aux);
       var_update(keep_steps);
       bar();
     }
@@ -2782,7 +2513,7 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
       }
     }
     // long trajectories / wide blocks: rows in shared memory -> the plain block; rows in global memory -> column-major copy
-    BlockFn volatile fn = q.rows_smem ? &admm_block<NB, PAIR, false> : &admm_block_soa<NB, PAIR>;
+    BlockFn volatile fn = q.rows_smem ? &admm_block<NB, PAIR> : &admm_block_soa<NB, PAIR>;
     fn(q, sysw.rho_aux, n, keep_last ? 1 : 0);
   };
   // the same for the factorisation (a few calls per QP, tens of thousands of cycles each); the polish system always
