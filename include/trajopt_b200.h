@@ -30,7 +30,7 @@ extern "C" {
 #endif
 
 #define TB200_VERSION_MAJOR 0
-#define TB200_VERSION_MINOR 4
+#define TB200_VERSION_MINOR 5
 #define TB200_MAX_DOF 16      /* joints per manipulator group (7 single arm, 14 dual arm) */
 #define TB200_MAX_STEPS 64    /* waypoints per trajectory */
 #define TB200_MIN_CAST_ROWS_PER_PAIR 128  /* continuous collision evaluators: lower / upper limit of the active contacts */
@@ -415,6 +415,55 @@ typedef struct tb200_check_results {
  * fetch needs no round trip).  TB200_ERR_INVALID for an unknown type, an LVS type with lvs <= 0 or NaN, a non-finite
  * margin, and a NULL x before any solve. */
 int tb200_check_trajectories(tb200_problem* p, const double* x, const tb200_check_config* cfg, tb200_check_results* out);
+
+/* ---- SQP iteration log (DESIGN.md section 4.7) --------------------------------------------------------------------
+ * Opt-in record of what every trajectory's SQP did, written on the device by the decision step.  capacity R > 0: the
+ * next solves keep up to R records per trajectory (later ones are counted in n_dropped and not written, so the records
+ * kept are always the same prefix); with_x 1: each record also holds its point [T][D].  0: off (the default).  Takes
+ * effect at the next solve; the log of a solve stays readable until the next one.  TB200_ERR_INVALID for a negative
+ * capacity, a with_x other than 0 or 1, and a buffer (batch x R x record size) that cannot be addressed.  Solves with
+ * and without the log compute the same results, bit for bit; tb200_convexify_batch and tb200_qp_solve_batch write no
+ * records. */
+int tb200_problem_set_sqp_log(tb200_problem* p, int32_t capacity, int32_t with_x);
+
+/* The log of the last solve.  Per trajectory b, records r < n_records[b] in order: record 0 (kind 0) is the state after
+ * the initial evaluation (the clamped start point, its exact values, the initial merit coefficients and trust box);
+ * then one record (kind 1) per QP solve, failed ones included, in the order of n_qp_solves.  A trajectory ended by the
+ * time limit or by its group simply has no more records.  Arrays are [B][R](...) with R = the capacity the solve ran
+ * with; entries past n_records[b] are 0 / -1 / NaN.  Any pointer may be NULL to skip that output. */
+typedef struct tb200_sqp_log {
+  int32_t* n_records;       /* [B] records kept (n_qp_solves + 1 when nothing was dropped) */
+  int32_t* n_dropped;       /* [B] records that did not fit */
+  int32_t* kind;            /* [B][R] 0 initial state, 1 QP solve */
+  int32_t* merit_round;     /* [B][R] merit coefficient round the QP belongs to (0-based) */
+  int32_t* iter;            /* [B][R] SQP iteration within that round (1-based) */
+  double* trust_box_size;   /* [B][R] trust box the QP was solved with (kind 0: the initial one) */
+  int32_t* qp_status;       /* [B][R] QP solver status (OSQP's values, see tb200_qp_solve_general); -1 for kind 0 */
+  int32_t* admm_iters;      /* [B][R] ADMM iterations of the QP */
+  int32_t* polish;          /* [B][R] 1 polish accepted, -1 rejected, 0 not attempted */
+  double* qp_diag;          /* [B][R][4] primal residual, dual residual, final rho, 1 if warm started */
+  int32_t* action;          /* [B][R] 0 trust box shrunk, 1 step accepted, 2 converged by small improvement, 3 QP
+                               failure; -1 for kind 0 */
+  int32_t* ended;           /* [B][R] TB200_OPT_* the trajectory ended with at this record, -1: it went on */
+  double* old_merit;        /* [B][R] merit at the last accepted point; NaN for kind 0 and a failed QP */
+  double* model_merit;      /* [B][R] merit of the QP model at its solution; NaN likewise */
+  double* new_merit;        /* [B][R] exact merit at the QP solution; NaN likewise */
+  double* merit_coeffs;     /* [B][R][n_cnts] merit coefficients the decision used */
+  double* model_cost_vals;  /* [B][R][n_costs] model value of every cost at the QP solution, as summed into model_merit */
+  double* model_cnt_viols;  /* [B][R][n_cnts] NaN for kind 0 and a failed QP */
+  double* old_cost_vals;    /* [B][R][n_costs] exact values at the last accepted point (filled on the host) */
+  double* old_cnt_viols;    /* [B][R][n_cnts]  NaN for kind 0 */
+  double* new_cost_vals;    /* [B][R][n_costs] exact values at the record's point (kind 0: the start; NaN: failed QP) */
+  double* new_cnt_viols;    /* [B][R][n_cnts] */
+  double* new_x;            /* [B][R][T][D] the record's point; only when the log was recorded with_x */
+} tb200_sqp_log;
+int tb200_fetch_sqp_log(tb200_problem* p, tb200_sqp_log* out);
+
+/* The sco::Cost / sco::Constraint objects of the problem in OptProb order (costs, then equality constraints, then
+ * inequality constraints: the order of cost_vals and cnt_viols): term[i] = index in desc.terms of the term that hatched
+ * object i, step[i] = its step (joint terms: their first step; collision and CartVel: the step or first step of the
+ * pair).  n_costs + n_cnts entries each (tb200_problem_layout); either pointer may be NULL. */
+int tb200_problem_objects(const tb200_problem* p, int32_t* term, int32_t* step);
 
 /* Timing of the last tb200_solve_batch* call, measured with CUDA events on the solver's
  * stream: total ms, convexify-kernel ms and launches, qp-kernel ms and launches. */

@@ -17,8 +17,14 @@
 // Header only; link with -ltrajopt_b200.  Everything lives in namespace trajopt_b200 so that a shim inside the
 // reference tree can alias it (namespace tb = trajopt_b200).
 #pragma once
+#include <algorithm>
 #include <cmath>
 #include <cstdint>
+#include <cstdio>
+#include <filesystem>
+#include <fstream>
+#include <functional>
+#include <map>
 #include <limits>
 #include <memory>
 #include <stdexcept>
@@ -61,6 +67,10 @@ struct BasicTrustRegionSQPParameters {
   bool inflate_constraints_individually = true;
   double trust_box_size = 1e-1;
   double max_time = std::numeric_limits<double>::max();  // seconds (DESIGN.md section 6: one device clock per batch)
+  // optimizers.hpp:127-129: write log_dir/<problem>/trajopt_{solver,vars,costs,constraints}.log (OptimizeWithParams from
+  // pci.opt_info or with callbacks; one directory per problem of the batch).  Not read from JSON, as in the reference.
+  bool log_results = false;
+  std::string log_dir = "/tmp";
 };
 
 // optimizers.hpp:40-59
@@ -315,6 +325,10 @@ struct FlatProblem {
   std::vector<tb200_term> terms;
   std::vector<int32_t> fixed_timesteps, fixed_dofs;
   int n_costs_terms = 0;
+  std::vector<std::string> term_names;  // TermInfo::name of every term, in terms order
+  bool log_results = false;             // pci.opt_info.log_results / log_dir
+  std::string log_dir;
+  std::shared_ptr<const RobotModel> kin;  // pci.kin (WriteCallback's FK)
 };
 
 // The part of ConstructProblem (problem_description.cpp:410-542) that does not need the device: checks, initial
@@ -380,6 +394,11 @@ inline std::shared_ptr<FlatProblem> FlattenProblem(const ProblemConstructionInfo
     if (ti->term_type != TT_CNT) throw std::runtime_error(ti->name + ": a cnt_info must have term_type TT_CNT");
     ti->hatch(flat, pci);
   }
+  for (const auto* infos : {&pci.cost_infos, &pci.cnt_infos})
+    for (const auto& ti : *infos) fp->term_names.push_back(ti->name);  // (every hatch adds one term)
+  fp->log_results = pci.opt_info.log_results;
+  fp->kin = pci.kin;
+  fp->log_dir = pci.opt_info.log_dir;
   fp->terms = flat.terms;
   fp->cart_targets = flat.cart_targets;
   {
@@ -456,6 +475,7 @@ public:
   int getNumCosts() const { return layout_.n_costs; }
   int getNumConstraints() const { return layout_.n_cnts; }
   tb200_problem* handle() const { return handle_; }
+  const FlatProblem& flat() const { return *flat_; }
 
 private:
   std::shared_ptr<FlatProblem> flat_;
@@ -494,8 +514,9 @@ inline std::vector<sco::OptResults> OptimizeWithParams(TrajOptProb& prob, const 
   }
   return out;
 }
-// ... with the problem description's own parameters (pci.opt_info)
-inline std::vector<sco::OptResults> OptimizeWithParams(TrajOptProb& prob) { return OptimizeWithParams(prob, prob.sqpParams()); }
+// ... with the problem description's own parameters (pci.opt_info; with its log_results, log_dir/<problem>/trajopt_*.log
+// are written as by the overload with callbacks)
+inline std::vector<sco::OptResults> OptimizeWithParams(TrajOptProb& prob);
 
 // trajopt::OptimizeProblem(prob) (problem_description.hpp:665, problem_description.cpp:392-408).  The reference's function
 // does NOT run with pci.opt_info: it builds a fresh BasicTrustRegionSQP and overrides four parameters (max_iter 40,
@@ -510,6 +531,370 @@ inline std::vector<sco::OptResults> OptimizeProblem(TrajOptProb& prob) {
   p.improve_ratio_threshold = .2;
   p.initial_merit_error_coeff = 20;
   return OptimizeWithParams(prob, p);
+}
+
+// ---- SQP iteration log, optimizer callbacks and log_results (DESIGN.md section 4.7) ----------------------------------
+
+// The log of the last solve (tb200_fetch_sqp_log) on the host: R records per problem, [B][R](...) like the C struct.
+struct SqpLog {
+  int B = 0, R = 0, n_costs = 0, n_cnts = 0, N = 0;
+  bool with_x = false;
+  std::vector<int32_t> n_records, n_dropped, kind, merit_round, iter, qp_status, admm_iters, polish, action, ended;
+  DblVec trust_box_size, old_merit, model_merit, new_merit, merit_coeffs, model_cost_vals, model_cnt_viols, old_cost_vals,
+      old_cnt_viols, new_cost_vals, new_cnt_viols, new_x;
+  size_t at(size_t b, size_t r) const { return b * R + r; }
+};
+
+inline SqpLog FetchSqpLog(TrajOptProb& prob, int capacity, bool with_x) {
+  SqpLog L;
+  L.B = prob.GetBatch(); L.R = capacity; L.n_costs = prob.getNumCosts(); L.n_cnts = prob.getNumConstraints();
+  L.N = prob.GetNumSteps() * prob.GetNumDOF(); L.with_x = with_x;
+  const size_t BR = static_cast<size_t>(L.B) * L.R;
+  for (auto* v : {&L.kind, &L.merit_round, &L.iter, &L.qp_status, &L.admm_iters, &L.polish, &L.action, &L.ended}) v->resize(BR);
+  for (auto* v : {&L.trust_box_size, &L.old_merit, &L.model_merit, &L.new_merit}) v->resize(BR);
+  L.n_records.resize(L.B); L.n_dropped.resize(L.B);
+  L.merit_coeffs.resize(BR * L.n_cnts); L.model_cnt_viols.resize(BR * L.n_cnts); L.old_cnt_viols.resize(BR * L.n_cnts);
+  L.new_cnt_viols.resize(BR * L.n_cnts);
+  L.model_cost_vals.resize(BR * L.n_costs); L.old_cost_vals.resize(BR * L.n_costs); L.new_cost_vals.resize(BR * L.n_costs);
+  if (with_x) L.new_x.resize(BR * L.N);
+  auto p = [](DblVec& v) { return v.empty() ? nullptr : v.data(); };
+  tb200_sqp_log o{};
+  o.n_records = L.n_records.data(); o.n_dropped = L.n_dropped.data(); o.kind = L.kind.data();
+  o.merit_round = L.merit_round.data(); o.iter = L.iter.data(); o.trust_box_size = p(L.trust_box_size);
+  o.qp_status = L.qp_status.data(); o.admm_iters = L.admm_iters.data(); o.polish = L.polish.data();
+  o.action = L.action.data(); o.ended = L.ended.data();
+  o.old_merit = p(L.old_merit); o.model_merit = p(L.model_merit); o.new_merit = p(L.new_merit);
+  o.merit_coeffs = p(L.merit_coeffs); o.model_cost_vals = p(L.model_cost_vals); o.model_cnt_viols = p(L.model_cnt_viols);
+  o.old_cost_vals = p(L.old_cost_vals); o.old_cnt_viols = p(L.old_cnt_viols);
+  o.new_cost_vals = p(L.new_cost_vals); o.new_cnt_viols = p(L.new_cnt_viols); o.new_x = p(L.new_x);
+  if (tb200_fetch_sqp_log(prob.handle(), &o) != TB200_OK) throw std::runtime_error(tb200_last_error());
+  return L;
+}
+
+// sco::Optimizer::Callback (optimizers.hpp:83) for a batch: the problem index says whose state the results are.
+using Callback = std::function<void(TrajOptProb*, std::size_t problem, sco::OptResults&)>;
+
+// Calls the callbacks as the reference's optimizer does for problem b (optimizers.cpp:754, 978): once at the top of every
+// SQP iteration that ran a QP - a new (merit_round, iter) in the log - and once at the end with final.  At a top the
+// results hold what the reference's hold there: the last accepted point and its exact values, and the QP solves and
+// function evaluations so far (a failed QP evaluates nothing); at the first top, before the first evaluation, the value
+// vectors are empty and the counts 0.  The log must hold the points (with_x).  A truncated log throws, naming the
+// problem, unless allow_truncated (then the replay stops with the records kept).
+inline void ReplayCallbacks(TrajOptProb* prob, const SqpLog& L, std::size_t b, sco::OptResults final_results,
+                            const std::vector<Callback>& callbacks, bool allow_truncated = false) {
+  if (L.n_dropped[b] > 0 && !allow_truncated)
+    throw std::runtime_error("SQP log of problem " + std::to_string(b) + " is truncated: " + std::to_string(L.n_dropped[b]) +
+                             " records did not fit a capacity of " + std::to_string(L.R));
+  if (!L.with_x) throw std::runtime_error("replaying callbacks needs a log recorded with x");
+  const size_t N = L.N, nc = L.n_costs, nk = L.n_cnts;
+  sco::OptResults cur;
+  cur.status = sco::INVALID;
+  int last_round = -1, last_iter = -1, n_qp = 0, n_fe = 0;
+  for (int r = 0; r < L.n_records[b]; ++r) {
+    const size_t i = L.at(b, r);
+    if (L.kind[i] == 0) {  // the state after the first evaluation: the first top sees its point, no values yet
+      cur.x.assign(L.new_x.begin() + i * N, L.new_x.begin() + (i + 1) * N);
+      continue;
+    }
+    if (L.merit_round[i] != last_round || L.iter[i] != last_iter) {
+      last_round = L.merit_round[i];
+      last_iter = L.iter[i];
+      cur.n_qp_solves = n_qp;
+      cur.n_func_evals = n_fe;
+      for (const Callback& cb : callbacks) {
+        sco::OptResults view = cur;
+        cb(prob, b, view);
+      }
+    }
+    if (n_fe == 0) {  // the first iteration evaluates the start point (optimizers.cpp:761-767)
+      const size_t i0 = L.at(b, 0);
+      cur.cost_vals.assign(L.new_cost_vals.begin() + i0 * nc, L.new_cost_vals.begin() + (i0 + 1) * nc);
+      cur.cnt_viols.assign(L.new_cnt_viols.begin() + i0 * nk, L.new_cnt_viols.begin() + (i0 + 1) * nk);
+      n_fe = 1;
+    }
+    ++n_qp;
+    if (L.action[i] != 3) ++n_fe;
+    if (L.action[i] == 1) {
+      cur.x.assign(L.new_x.begin() + i * N, L.new_x.begin() + (i + 1) * N);
+      cur.cost_vals.assign(L.new_cost_vals.begin() + i * nc, L.new_cost_vals.begin() + (i + 1) * nc);
+      cur.cnt_viols.assign(L.new_cnt_viols.begin() + i * nk, L.new_cnt_viols.begin() + (i + 1) * nk);
+    }
+  }
+  for (const Callback& cb : callbacks) {
+    sco::OptResults view = final_results;
+    cb(prob, b, view);
+  }
+}
+
+// Names the reference gives the variables (problem_description.cpp:573-578) and the objects (TermInfo::hatch: the term's
+// name; collision objects "<name>_<step>", :1758-1832).
+inline std::vector<std::string> VarNames(int T, int D) {
+  std::vector<std::string> v;
+  for (int t = 0; t < T; ++t)
+    for (int d = 0; d < D; ++d) v.push_back("j_" + std::to_string(t) + "_" + std::to_string(d));
+  return v;
+}
+inline void ObjectNames(const TrajOptProb& prob, std::vector<std::string>& cost_names, std::vector<std::string>& cnt_names) {
+  const int nc = prob.getNumCosts(), nk = prob.getNumConstraints();
+  std::vector<int32_t> term(nc + nk + 1), step(nc + nk + 1);
+  if (tb200_problem_objects(prob.handle(), term.data(), step.data()) != TB200_OK) throw std::runtime_error(tb200_last_error());
+  const FlatProblem& f = prob.flat();
+  cost_names.clear();
+  cnt_names.clear();
+  for (int i = 0; i < nc + nk; ++i) {
+    const tb200_term& t = f.terms[term[i]];
+    std::string n = f.term_names[term[i]];
+    if (t.kind == TB200_TERM_COLLISION) n += "_" + std::to_string(step[i]);
+    if (t.kind == TB200_TERM_CART_VEL && t.role == TB200_ROLE_CNT) n = "CartVel";  // :1044-1052 names its constraints so
+    (i < nc ? cost_names : cnt_names).push_back(n);
+  }
+}
+
+// log_results for problem b: dir/trajopt_{solver,vars,costs,constraints}.log, one line per successful QP with the header
+// before the first, in the reference's formats (BasicTrustRegionSQPResults::write*, optimizers.cpp:533-647).
+inline void WriteLogResults(const SqpLog& L, std::size_t b, const std::string& dir, const std::vector<std::string>& var_names,
+                            const std::vector<std::string>& cost_names, const std::vector<std::string>& cnt_names) {
+  std::filesystem::create_directories(dir);
+  const char* files[4] = {"/trajopt_solver.log", "/trajopt_vars.log", "/trajopt_costs.log", "/trajopt_constraints.log"};
+  std::FILE* f[4];
+  for (int k = 0; k < 4; ++k)
+    if (!(f[k] = std::fopen((dir + files[k]).c_str(), "w"))) throw std::runtime_error("cannot open " + dir + files[k]);
+  const size_t N = L.N, nc = L.n_costs, nk = L.n_cnts;
+  bool header = true;
+  for (int r = 0; r < L.n_records[b]; ++r) {
+    const size_t i = L.at(b, r);
+    if (L.kind[i] != 1 || L.action[i] == 3) continue;  // the reference logs successful QPs only
+    const double old_m = L.old_merit[i], model_m = L.model_merit[i], new_m = L.new_merit[i];
+    const double approx = old_m - model_m, exact = old_m - new_m;
+    if (header) std::fprintf(f[0], "%s,%s,%s,%s,%s,%s\n", "DESCRIPTION", "oldexact", "new_exact", "dapprox", "dexact", "ratio");
+    std::fprintf(f[0], "%s,%10.3e,%10.3e,%10.3e,%10.3e,%10.3e\n", "Solver", old_m, new_m, approx, exact, exact / approx);
+    if (header) {
+      std::fprintf(f[1], "%s", "NAMES");
+      for (const auto& v : var_names) std::fprintf(f[1], ",%s", v.c_str());
+      std::fprintf(f[1], "\n");
+    }
+    std::fprintf(f[1], "%s", "VALUES");
+    for (size_t k = 0; k < N && L.with_x; ++k) std::fprintf(f[1], ",%e", L.new_x[i * N + k]);
+    std::fprintf(f[1], "\n");
+    // costs (scale 1) and constraints (scaled by their merit coefficients)
+    for (int c = 0; c < 2; ++c) {
+      std::FILE* s = f[2 + c];
+      const std::vector<std::string>& names = c ? cnt_names : cost_names;
+      const size_t n = c ? nk : nc;
+      const double* o = (c ? L.old_cnt_viols.data() : L.old_cost_vals.data()) + i * n;
+      const double* m = (c ? L.model_cnt_viols.data() : L.model_cost_vals.data()) + i * n;
+      const double* w = (c ? L.new_cnt_viols.data() : L.new_cost_vals.data()) + i * n;
+      if (header) {
+        std::fprintf(s, "%s", c ? "CONSTRAINT NAMES" : "COST NAMES");
+        for (const auto& nm : names) std::fprintf(s, ",%s,%s,%s,%s", nm.c_str(), nm.c_str(), nm.c_str(), nm.c_str());
+        std::fprintf(s, "\n");
+        std::fprintf(s, "%s", "DESCRIPTION");
+        for (size_t k = 0; k < names.size(); ++k) std::fprintf(s, ",%s,%s,%s,%s", "oldexact", "dapprox", "dexact", "ratio");
+        std::fprintf(s, "\n");
+      }
+      std::fprintf(s, "%s", c ? "CONSTRAINTS" : "COSTS");
+      for (size_t k = 0; k < n; ++k) {
+        const double a = o[k] - m[k], e = o[k] - w[k], mu = c ? L.merit_coeffs[i * nk + k] : 1.0;
+        const double ov = c ? mu * o[k] : o[k], av = c ? mu * a : a, ev = c ? mu * e : e;
+        if (std::fabs(a) > 1e-8) std::fprintf(s, ",%e,%e,%e,%e", ov, av, ev, e / a);
+        else std::fprintf(s, ",%e,%e,%e,%s", ov, av, ev, "nan");
+      }
+      std::fprintf(s, "\n");
+    }
+    header = false;
+  }
+  for (std::FILE* s : f) std::fclose(s);
+}
+
+// OptimizeWithParams with callbacks: the batch is solved with the SQP log on (with the points), then, per problem in
+// batch order, the callbacks are replayed (ReplayCallbacks) and, with pci.opt_info's log_results,
+// log_dir/<problem>/trajopt_*.log written.  The results are those of the solve without the log, bit for bit.
+// log_capacity: records per problem; 0 sizes it from the parameters, 1 + max_iter x max_merit_coeff_increases (one QP per
+// SQP iteration).  The device holds batch x capacity x (16 + 2 n_costs + 3 n_cnts + T*D) doubles while the log is on,
+// and the host a copy of it: at configs[2] (batch 1024, 30 x 7 variables, 16 objects) 2560 bytes a record, 0.66 GB for
+// the default 251 records.  When a problem needed more, the batch is solved once more with exactly the capacity the log
+// counted (the solve is deterministic), unless allow_truncated asks for the prefix.
+namespace detail {
+inline std::vector<sco::OptResults> optimizeLogged(TrajOptProb& prob, const tb200_sqp_params& params,
+                                                   const std::vector<Callback>& callbacks, bool log_results,
+                                                   int log_capacity, bool allow_truncated);
+}
+inline std::vector<sco::OptResults> OptimizeWithParams(TrajOptProb& prob, const tb200_sqp_params& params,
+                                                       const std::vector<Callback>& callbacks, int log_capacity = 0,
+                                                       bool allow_truncated = false) {
+  return detail::optimizeLogged(prob, params, callbacks, prob.flat().log_results, log_capacity, allow_truncated);
+}
+inline std::vector<sco::OptResults> detail::optimizeLogged(TrajOptProb& prob, const tb200_sqp_params& params,
+                                                           const std::vector<Callback>& callbacks, bool log_results,
+                                                           int log_capacity, bool allow_truncated) {
+  int cap = log_capacity > 0 ? log_capacity
+                             : 1 + std::max(params.max_iter, 1) * static_cast<int>(std::ceil(std::max(params.max_merit_coeff_increases, 1.0)));
+  std::vector<sco::OptResults> out;
+  SqpLog L;
+  try {
+    for (;;) {
+      if (tb200_problem_set_sqp_log(prob.handle(), cap, 1) != TB200_OK) throw std::runtime_error(tb200_last_error());
+      out = OptimizeWithParams(prob, params);
+      L = FetchSqpLog(prob, cap, true);
+      int need = 0;
+      for (int b = 0; b < L.B; ++b) need = std::max(need, L.n_records[b] + L.n_dropped[b]);
+      if (need <= cap || allow_truncated) break;
+      cap = need;
+    }
+  } catch (...) {
+    tb200_problem_set_sqp_log(prob.handle(), 0, 0);
+    throw;
+  }
+  tb200_problem_set_sqp_log(prob.handle(), 0, 0);
+  std::vector<std::string> var_names, cost_names, cnt_names;
+  if (log_results) {
+    var_names = VarNames(prob.GetNumSteps(), prob.GetNumDOF());
+    ObjectNames(prob, cost_names, cnt_names);
+  }
+  for (size_t b = 0; b < out.size(); ++b) {
+    ReplayCallbacks(&prob, L, b, out[b], callbacks, allow_truncated);
+    if (log_results) WriteLogResults(L, b, prob.flat().log_dir + "/" + std::to_string(b), var_names, cost_names, cnt_names);
+  }
+  return out;
+}
+// ... with the problem description's own parameters (pci.opt_info, its log_results and log_dir included)
+inline std::vector<sco::OptResults> OptimizeWithParams(TrajOptProb& prob, const std::vector<Callback>& callbacks) {
+  return OptimizeWithParams(prob, prob.sqpParams(), callbacks);
+}
+// trajopt::OptimizeProblem with callbacks attached (problem_description.cpp:396-404 attaches its PlotCallback the same way);
+// its fresh parameters keep the default log_results = false, as the reference's do
+inline std::vector<sco::OptResults> OptimizeProblem(TrajOptProb& prob, const std::vector<Callback>& callbacks) {
+  tb200_sqp_params p;
+  tb200_default_sqp_params(&p);
+  p.max_iter = 40;
+  p.min_approx_improve_frac = .001;
+  p.improve_ratio_threshold = .2;
+  p.initial_merit_error_coeff = 20;
+  return detail::optimizeLogged(prob, p, callbacks, false, 0, false);
+}
+inline std::vector<sco::OptResults> OptimizeWithParams(TrajOptProb& prob) {
+  if (prob.flat().log_results) return detail::optimizeLogged(prob, prob.sqpParams(), {}, true, 0, false);
+  return OptimizeWithParams(prob, prob.sqpParams());
+}
+
+// The frames of every link of a RobotModel at joint values q: the arithmetic of the test oracle's Robot::fk (origin
+// quaternion -> rotation, Rodrigues for a revolute joint, axis * q for a prismatic one, parent frame * origin * motion),
+// restated here.  frames[j] is the frame the joint j creates (RobotModel::joints order): R row-major, then p.
+struct Frame {
+  double R[9];
+  double p[3];
+};
+inline std::vector<Frame> RobotFK(const RobotModel& kin, const double* q) {
+  auto mul = [](const Frame& a, const Frame& b) {
+    Frame o{};
+    for (int i = 0; i < 3; ++i) {
+      for (int j = 0; j < 3; ++j) {
+        double s = 0;
+        for (int k = 0; k < 3; ++k) s += a.R[i * 3 + k] * b.R[k * 3 + j];
+        o.R[i * 3 + j] = s;
+      }
+      o.p[i] = a.R[i * 3] * b.p[0] + a.R[i * 3 + 1] * b.p[1] + a.R[i * 3 + 2] * b.p[2] + a.p[i];
+    }
+    return o;
+  };
+  std::vector<Frame> f(kin.joints.size());
+  for (size_t s = 0; s < kin.joints.size(); ++s) {
+    const RobotModel::Joint& g = kin.joints[s];
+    Frame t{};
+    double w = g.origin.wxyz[0], x = g.origin.wxyz[1], y = g.origin.wxyz[2], z = g.origin.wxyz[3];
+    const double n = std::sqrt(w * w + x * x + y * y + z * z);
+    w /= n; x /= n; y /= n; z /= n;
+    t.R[0] = 1 - 2 * (y * y + z * z); t.R[1] = 2 * (x * y - z * w);     t.R[2] = 2 * (x * z + y * w);
+    t.R[3] = 2 * (x * y + z * w);     t.R[4] = 1 - 2 * (x * x + z * z); t.R[5] = 2 * (y * z - x * w);
+    t.R[6] = 2 * (x * z - y * w);     t.R[7] = 2 * (y * z + x * w);     t.R[8] = 1 - 2 * (x * x + y * y);
+    for (int i = 0; i < 3; ++i) t.p[i] = g.origin.xyz[i];
+    if (g.type == TB200_JOINT_REVOLUTE) {
+      const double a = q[g.q_index], c = std::cos(a), sn = std::sin(a), v = 1 - c;
+      const double ax = g.axis[0], ay = g.axis[1], az = g.axis[2];
+      Frame m{};
+      m.R[0] = c + ax * ax * v;      m.R[1] = ax * ay * v - az * sn; m.R[2] = ax * az * v + ay * sn;
+      m.R[3] = ay * ax * v + az * sn; m.R[4] = c + ay * ay * v;      m.R[5] = ay * az * v - ax * sn;
+      m.R[6] = az * ax * v - ay * sn; m.R[7] = az * ay * v + ax * sn; m.R[8] = c + az * az * v;
+      t = mul(t, m);
+    } else if (g.type == TB200_JOINT_PRISMATIC) {
+      Frame m{};
+      m.R[0] = m.R[4] = m.R[8] = 1.0;
+      for (int i = 0; i < 3; ++i) m.p[i] = g.axis[i] * q[g.q_index];
+      t = mul(t, m);
+    }
+    f[s] = (g.parent < 0) ? t : mul(f[g.parent], t);
+  }
+  return f;
+}
+// Eigen::Quaterniond(Matrix3d) of a row-major rotation, (w, x, y, z): the trace branch and the largest-diagonal branch.
+inline void RotToQuatWxyz(const double* m, double* q) {
+  double t = m[0] + m[4] + m[8];
+  if (t > 0) {
+    t = std::sqrt(t + 1.0);
+    q[0] = 0.5 * t;
+    t = 0.5 / t;
+    q[1] = (m[7] - m[5]) * t;
+    q[2] = (m[2] - m[6]) * t;
+    q[3] = (m[3] - m[1]) * t;
+  } else {
+    int i = 0;
+    if (m[4] > m[0]) i = 1;
+    if (m[8] > m[i * 3 + i]) i = 2;
+    const int j = (i + 1) % 3, k = (j + 1) % 3;
+    t = std::sqrt(m[i * 3 + i] - m[j * 3 + j] - m[k * 3 + k] + 1.0);
+    q[1 + i] = 0.5 * t;
+    t = 0.5 / t;
+    q[0] = (m[k * 3 + j] - m[j * 3 + k]) * t;
+    q[1 + j] = (m[j * 3 + i] + m[i * 3 + j]) * t;
+    q[1 + k] = (m[k * 3 + i] + m[i * 3 + k]) * t;
+  }
+}
+
+// trajopt::WriteCallback (file_write_callback.cpp) for the batch.  On creation it writes the header line: the joint names
+// (here the child link of each moving joint, in column order), x,y,z,q_w,q_x,q_y,q_z, the cost names and the constraint
+// names.  Every call then writes, per waypoint of the problem's x, a line of the joint values, then for every link of
+// the model "<link>: " and ",x,y,z,qw,qx,qy,qz" of its frame (the reference iterates tesseract's TransformMap, an unordered
+// map; here the links go in name order), then ",<cost>" per cost value and ",<violation>" per constraint value; and
+// an empty line after the last waypoint.  Numbers go through operator<< as in the reference.  The problem index of the
+// batch is not written: with several problems the blocks follow in call order.
+inline Callback WriteCallback(std::shared_ptr<std::ofstream> file, std::shared_ptr<const RobotModel> kin,
+                              const std::vector<std::string>& cost_names, const std::vector<std::string>& cnt_names) {
+  if (!file->good()) std::fprintf(stderr, "ofstream passed to create callback not in 'good' state\n");
+  std::vector<std::string> joint_names(kin->numJoints());
+  for (const RobotModel::Joint& j : kin->joints)
+    if (j.type != TB200_JOINT_FIXED && j.q_index >= 0 && j.q_index < kin->numJoints()) joint_names[j.q_index] = j.child_link;
+  for (size_t i = 0; i < joint_names.size(); ++i) *file << (i ? "," : "") << joint_names[i];
+  for (const char* s : {"x", "y", "z", "q_w", "q_x", "q_y", "q_z"}) *file << ',' << s;
+  for (const auto& n : cost_names) *file << ',' << n;
+  for (const auto& n : cnt_names) *file << ',' << n;
+  *file << '\n' << std::flush;
+  const int D = kin->numJoints();
+  return [file, kin, D](TrajOptProb*, std::size_t, sco::OptResults& r) {
+    std::map<std::string, size_t> links;  // name order
+    for (size_t s = 0; s < kin->joints.size(); ++s) links.emplace(kin->joints[s].child_link, s);
+    const size_t T = D ? r.x.size() / D : 0;
+    for (size_t t = 0; t < T; ++t) {
+      const double* q = r.x.data() + t * D;
+      for (int j = 0; j < D; ++j) *file << (j ? "," : "") << q[j];
+      const std::vector<Frame> fr = RobotFK(*kin, q);
+      for (const auto& [name, s] : links) {
+        double wxyz[4];
+        RotToQuatWxyz(fr[s].R, wxyz);
+        *file << name << ": ";
+        for (double v : {fr[s].p[0], fr[s].p[1], fr[s].p[2], wxyz[0], wxyz[1], wxyz[2], wxyz[3]}) *file << ',' << v;
+      }
+      for (double c : r.cost_vals) *file << ',' << c;
+      for (double c : r.cnt_viols) *file << ',' << c;
+      *file << '\n';
+    }
+    *file << '\n' << std::flush;
+  };
+}
+// ... for a problem: its robot model (pci.kin) and its object names (ObjectNames)
+inline Callback WriteCallback(std::shared_ptr<std::ofstream> file, const TrajOptProb& prob) {
+  std::vector<std::string> cost_names, cnt_names;
+  ObjectNames(prob, cost_names, cnt_names);
+  return WriteCallback(std::move(file), prob.flat().kin, cost_names, cnt_names);
 }
 
 // One problem of a multi-start solve (ProblemConstructionInfo::seeds_per_problem): its best seed and what every seed did.

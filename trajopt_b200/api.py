@@ -33,6 +33,8 @@ class Problem:
         self._check(self.lib.tb200_problem_layout(self.handle, C.byref(self.layout)))
         self.group_size = max(desc.c.group_size, 1)
         self._solved_group_size = None
+        self._log_shape = (0, False)
+        self._solved_log_shape = None
 
     def _check(self, rc):
         if rc != 0:
@@ -77,6 +79,43 @@ class Problem:
         self._check(self.lib.tb200_fetch_group_results(self.handle, C.byref(r)))
         return out
 
+    def set_sqp_log(self, capacity, with_x=False):
+        """Record the SQP iteration log of the next solves: up to `capacity` records per trajectory (the state after the
+        initial evaluation, then one per QP solve), each with its point when with_x.  capacity 0 turns it off."""
+        self._check(self.lib.tb200_problem_set_sqp_log(self.handle, int(capacity), 1 if with_x else 0))
+        self._log_shape = (int(capacity), bool(with_x))
+
+    def sqp_log(self):
+        """The SQP iteration log of the last solve as a dict of numpy arrays (fields of tb200_sqp_log, [B][R](...)).
+        Per-record arrays hold NaN / 0 / -1 past n_records[b]; new_x is present only for a log recorded with x."""
+        L, d = self.layout, self.desc
+        R, with_x = self._solved_log_shape or (0, False)
+        B, nc, nk = d.B, L.n_costs, L.n_cnts
+        out = dict(n_records=np.zeros(B, np.int32), n_dropped=np.zeros(B, np.int32))
+        for k in ("kind", "merit_round", "iter", "qp_status", "admm_iters", "polish", "action", "ended"):
+            out[k] = np.zeros((B, R), np.int32)
+        for k in ("trust_box_size", "old_merit", "model_merit", "new_merit"):
+            out[k] = np.zeros((B, R))
+        out["qp_diag"] = np.zeros((B, R, 4))
+        out["merit_coeffs"] = np.zeros((B, R, nk))
+        for k, n in (("model_cost_vals", nc), ("model_cnt_viols", nk), ("old_cost_vals", nc), ("old_cnt_viols", nk),
+                     ("new_cost_vals", nc), ("new_cnt_viols", nk)):
+            out[k] = np.zeros((B, R, n))
+        if with_x:
+            out["new_x"] = np.zeros((B, R, d.T, d.D))
+        r = capi.SqpLog(*[(_ip if out[k].dtype == np.int32 else _dp)(out[k]) if k in out and out[k].size else None
+                          for k, _ in capi.SqpLog._fields_])
+        self._check(self.lib.tb200_fetch_sqp_log(self.handle, C.byref(r)))
+        return out
+
+    def objects(self):
+        """Per cost / constraint object (costs, then constraints, the order of cost_vals / cnt_viols): the index of
+        the term that hatched it and its step."""
+        n = self.layout.n_costs + self.layout.n_cnts
+        term, step = np.zeros(max(n, 1), np.int32), np.zeros(max(n, 1), np.int32)
+        self._check(self.lib.tb200_problem_objects(self.handle, _ip(term), _ip(step)))
+        return term[:n], step[:n]
+
     def _results(self):
         L, d = self.layout, self.desc
         return capi.alloc_results(d.B, d.T, d.D, L.n_costs, L.n_cnts)
@@ -85,12 +124,14 @@ class Problem:
         """BasicTrustRegionSQP::optimize() for the whole batch; host buffers in and out."""
         buf, res = self._results()
         self._solved_group_size = self.group_size
+        self._solved_log_shape = self._log_shape
         self._check(self.lib.tb200_solve_batch(self.handle, C.byref(res)))
         buf["timing"] = self.timing()
         return buf
 
     def solve_resident(self):
         self._solved_group_size = self.group_size
+        self._solved_log_shape = self._log_shape
         self._check(self.lib.tb200_solve_batch_resident(self.handle))
 
     def fetch(self):
@@ -171,18 +212,23 @@ class Problem:
         return out
 
 
-def solve(desc, device=0, group_size=None, group_stop=None):
+def solve(desc, device=0, group_size=None, group_stop=None, sqp_log=None, sqp_log_x=False):
     """One-shot: create, solve, destroy.  With group_size (and group_stop) the solve is a multi-start one
     (Problem.set_groups; None keeps the description's own settings) and the result gains a "groups" dict
-    (Problem.group_results)."""
+    (Problem.group_results).  With sqp_log = capacity the SQP iteration log is recorded (with the points when
+    sqp_log_x) and the result gains a "sqp_log" dict (Problem.sqp_log)."""
     p = Problem(desc, device)
     try:
         if group_size is not None or group_stop is not None:
             p.set_groups(desc.c.group_size if group_size is None else group_size,
                          desc.c.group_stop if group_stop is None else group_stop)
+        if sqp_log:
+            p.set_sqp_log(sqp_log, with_x=sqp_log_x)
         out = p.solve()
         if group_size is not None:
             out["groups"] = p.group_results()
+        if sqp_log:
+            out["sqp_log"] = p.sqp_log()
         return out
     finally:
         p.close()

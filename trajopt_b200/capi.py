@@ -119,6 +119,16 @@ class CheckResults(C.Structure):
                 ("in_collision", _i32_p), ("first_slot", _i32_p), ("min_distance", _dbl_p)]
 
 
+class SqpLog(C.Structure):
+    """tb200_sqp_log: the SQP iteration log of the last solve ([B][R](...) arrays, NULL-skippable)."""
+    _fields_ = [("n_records", _i32_p), ("n_dropped", _i32_p), ("kind", _i32_p), ("merit_round", _i32_p), ("iter", _i32_p),
+                ("trust_box_size", _dbl_p), ("qp_status", _i32_p), ("admm_iters", _i32_p), ("polish", _i32_p),
+                ("qp_diag", _dbl_p), ("action", _i32_p), ("ended", _i32_p), ("old_merit", _dbl_p), ("model_merit", _dbl_p),
+                ("new_merit", _dbl_p), ("merit_coeffs", _dbl_p), ("model_cost_vals", _dbl_p), ("model_cnt_viols", _dbl_p),
+                ("old_cost_vals", _dbl_p), ("old_cnt_viols", _dbl_p), ("new_cost_vals", _dbl_p), ("new_cnt_viols", _dbl_p),
+                ("new_x", _dbl_p)]
+
+
 class Timing(C.Structure):
     _fields_ = [("total_ms", C.c_double), ("convexify_ms", C.c_double), ("qp_ms", C.c_double),
                 ("merit_ms", C.c_double), ("convexify_launches", C.c_int32), ("qp_launches", C.c_int32),
@@ -290,6 +300,9 @@ def load_library():
     lib.tb200_problem_set_groups.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
     lib.tb200_fetch_group_results.argtypes = [C.c_void_p, C.POINTER(GroupResults)]
     lib.tb200_check_trajectories.argtypes = [C.c_void_p, _dbl_p, C.POINTER(CheckConfig), C.POINTER(CheckResults)]
+    lib.tb200_problem_set_sqp_log.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
+    lib.tb200_fetch_sqp_log.argtypes = [C.c_void_p, C.POINTER(SqpLog)]
+    lib.tb200_problem_objects.argtypes = [C.c_void_p, _i32_p, _i32_p]
     _LIB = lib
     return lib
 
@@ -301,4 +314,5 @@ EXPORTED_SYMBOLS = [
     "tb200_qp_solve_batch", "tb200_last_qp_polish", "tb200_last_timing",
     "tb200_qp_solve_general", "tb200_qp_general_last_error", "tb200_osqp_order_qp_settings", "tb200_problem_set_sqp_params",
     "tb200_problem_set_groups", "tb200_fetch_group_results", "tb200_check_trajectories",
+    "tb200_problem_set_sqp_log", "tb200_fetch_sqp_log", "tb200_problem_objects",
 ]

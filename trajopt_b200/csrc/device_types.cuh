@@ -160,4 +160,11 @@ struct DevProblem {
   SqpParams sqp;
 };
 
+// Record layout of the SQP iteration log: a header of kLogHeader doubles, then n_cnts merit coefficients, the model values
+// (n_costs, n_cnts), the exact values at the record's point (n_costs, n_cnts) and, with log_with_x, the point [T][D].
+enum LogField {
+  LOG_KIND = 0, LOG_ROUND, LOG_ITER, LOG_TRUST, LOG_OLD_MERIT, LOG_MODEL_MERIT, LOG_NEW_MERIT, LOG_QP_STATUS,
+  LOG_ADMM_ITERS, LOG_ACTION, LOG_PRI_RES, LOG_DUA_RES, LOG_RHO, LOG_POLISH, LOG_WARM, LOG_ENDED, kLogHeader
+};
+
 }  // namespace tb200

@@ -85,6 +85,13 @@ struct EvalExtra {
   const DevObj* coll_objs;
   int qtype[kMaxDof];                // joint type per trajectory column
   unsigned sphere_jmask[kMaxSpheres];  // which columns move each sphere
+  // SQP iteration log (tb200_problem_set_sqp_log; DESIGN.md section 4.7), nullptr: off.  One record per QP solve plus the
+  // state after the initial evaluation, [B][log_cap][log_stride] doubles; records past log_cap are counted, not written.
+  // (Here rather than in DevProblem: a larger DevProblem changes the register allocation of the QP step.)
+  double* log;
+  int* log_len;                // [B] records written
+  int* log_dropped;            // [B] records that did not fit
+  int log_cap, log_stride, log_with_x, pad;
 };
 
 #ifdef TB200_EVAL_PROFILE
@@ -153,6 +160,47 @@ __device__ __forceinline__ void cp_async8(double* smem_dst, const double* gsrc) 
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(d), "l"(gsrc) : "memory");
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// The SQP log record of a decision without its outcome (eval_step_impl; DESIGN.md section 4.7).  A function of its own so
+// that the decision code is compiled as without the log.
+static __device__ __noinline__ void log_record_arrays(const DevProblem& p, const EvalExtra& ex, const int mode, const int b,
+                                               const bool qp_failed, const DevObj* aobjs, const double* out_cost,
+                                               const double* out_viol, const double* xs) {
+  const int tid = threadIdx.x;
+  const int n = ex.log_len[b];
+  if (!(mode == EVAL_INIT || !(ex.cast && p.lvs_overflow[b])) || n >= ex.log_cap) return;
+  const double qnan = __longlong_as_double(0x7ff8000000000000ll);
+  const int nc = p.n_costs, nk = p.n_cnts;
+  double* rec = ex.log + (static_cast<size_t>(b) * ex.log_cap + n) * ex.log_stride;
+  if (tid == 0) {
+    const bool qp = mode == EVAL_STEP;
+    const double* g = p.dbg + static_cast<size_t>(b) * 16;
+    rec[LOG_KIND] = qp ? 1 : 0;
+    rec[LOG_ROUND] = p.merit_round[b]; rec[LOG_ITER] = p.sqp_iter[b]; rec[LOG_TRUST] = p.trust[b];
+    rec[LOG_OLD_MERIT] = rec[LOG_MODEL_MERIT] = rec[LOG_NEW_MERIT] = qnan;
+    rec[LOG_QP_STATUS] = qp ? g[0] : qnan; rec[LOG_ADMM_ITERS] = qp ? g[1] : qnan; rec[LOG_ACTION] = -1;
+    rec[LOG_PRI_RES] = qp ? g[4] : qnan; rec[LOG_DUA_RES] = qp ? g[5] : qnan; rec[LOG_RHO] = qp ? g[3] : qnan;
+    rec[LOG_POLISH] = qp ? g[2] : qnan; rec[LOG_WARM] = qp ? g[14] : qnan;
+  }
+  rec += kLogHeader;
+  const double* mu = p.merit_coeffs + static_cast<size_t>(b) * nk;
+  const double* mc = p.model_cost_vals + static_cast<size_t>(b) * nc;
+  const double* mk = p.model_cnt_viols + static_cast<size_t>(b) * nk;
+  const bool model = mode == EVAL_STEP && !qp_failed;
+  for (int i = tid; i < nk; i += kEvalThreads) rec[i] = mu[i];
+  rec += nk;
+  for (int i = tid; i < nc; i += kEvalThreads)  // as summed into model_merit: quadratic joint costs are exact
+    rec[i] = model ? (aobjs[i].kind == OBJ_JOINT_EQ_COST ? out_cost[i] : mc[i]) : qnan;
+  rec += nc;
+  for (int i = tid; i < nk; i += kEvalThreads) rec[i] = model ? mk[i] : qnan;
+  rec += nk;
+  for (int i = tid; i < nc; i += kEvalThreads) rec[i] = qp_failed ? qnan : out_cost[i];
+  rec += nc;
+  for (int i = tid; i < nk; i += kEvalThreads) rec[i] = qp_failed ? qnan : out_viol[i];
+  rec += nk;
+  if (ex.log_with_x)
+    for (int i = tid; i < p.N; i += kEvalThreads) rec[i] = qp_failed ? qnan : xs[i];
+}
 
 template <int DD>
 __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalExtra& ex, const int mode, const int b,
@@ -854,6 +902,17 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
   __threadfence_block();
   __syncthreads();
 
+  // ---- SQP iteration log (DESIGN.md section 4.7; off: one uniform branch) ----------------------------
+  // One record for the initial evaluation and one for every QP solve (the places n_qp_solves counts).  Everything but the
+  // decision's outcome goes out here, before the decision, because the penalty step below inflates the merit
+  // coefficients this decision used; thread 0 adds the merits, the action and the end status in the decision and only
+  // then counts the record (so the state machine keeps no log values live).  A failed QP has no model, point or values:
+  // NaN.
+  if (ex.log != nullptr) {
+    log_record_arrays(p, ex, mode, b, qp_failed, aobjs, out_cost, out_viol, xs);
+    __syncthreads();
+  }
+
   // ---- trust-region / penalty state machine (thread 0), optimizers.cpp:811-968 ----------------------
   if (tid == 0) {
     const SqpParams& sp = p.sqp;
@@ -933,6 +992,11 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
         te[6] = g[0]; te[7] = g[1]; te[8] = tr_action; te[9] = g[4]; te[10] = g[5]; te[11] = g[3]; te[12] = g[2]; te[13] = g[14];
         p.trace_len[b] += 1;
       }
+      if (ex.log != nullptr && ex.log_len[b] < ex.log_cap) {  // (the merits stay NaN for a failed QP)
+        double* lh = ex.log + (static_cast<size_t>(b) * ex.log_cap + ex.log_len[b]) * ex.log_stride;
+        if (!qp_failed) { lh[LOG_OLD_MERIT] = tr_old; lh[LOG_MODEL_MERIT] = tr_model; lh[LOG_NEW_MERIT] = tr_new; }
+        lh[LOG_ACTION] = tr_action;
+      }
       if (!finished && go == AFTER_LOOP) {
         const double* kk = accept ? out_viol : kv;
         if (trust < sp.min_trust_box_size) go = PENALTY;
@@ -970,6 +1034,15 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
             top = 1;
           }
         }
+      }
+    }
+    if (ex.log != nullptr && (mode == EVAL_INIT || !(ex.cast && p.lvs_overflow[b]))) {  // the record is complete
+      const int n = ex.log_len[b];
+      if (n < ex.log_cap) {
+        ex.log[(static_cast<size_t>(b) * ex.log_cap + n) * ex.log_stride + LOG_ENDED] = finished ? status : -1;
+        ex.log_len[b] = n + 1;
+      } else {
+        ex.log_dropped[b] += 1;
       }
     }
     p.trust[b] = trust;

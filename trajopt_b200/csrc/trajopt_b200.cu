@@ -92,6 +92,12 @@ struct tb200_problem {
   tb200_timing timing{};
   // host copies of the flattened description
   std::vector<DevObj> cost_objs, cnt_objs, cart_objs, coll_objs, vel_objs;
+  std::vector<std::pair<int, int>> obj_src;  // per object (costs, then constraints): the term that hatched it, its step
+  // SQP iteration log: the setting of the next solve, and the buffers of the last one (log_solved: it ran with the log)
+  int log_cap_next = 0, log_with_x_next = 0;
+  bool log_solved = false;
+  DevBuf<double> log;
+  DevBuf<int> log_len, log_dropped;
   bool pair_rows = false;  // QP rows span two waypoints (CartVel, continuous collision): 2*D coefficients per row
   // device storage
   DevBuf<DevSegment> segs;
@@ -136,12 +142,13 @@ struct tb200_problem {
     lists.release(); ws_meta.release(); tmp_iters.release(); tmp_polish.release();
     chk_slot_min.release(); chk_min.release(); chk_slot_contacts.release(); chk_slot_argmin.release(); chk_in_collision.release();
     chk_first.release();
+    log.release(); log_len.release(); log_dropped.release();
   }
 };
 
 extern "C" {
 
-const char* tb200_version(void) { return "trajopt_b200 0.4 (sm_90a)"; }
+const char* tb200_version(void) { return "trajopt_b200 0.5 (sm_90a)"; }
 const char* tb200_last_error(void) { return g_err.c_str(); }
 
 void tb200_default_sqp_params(tb200_sqp_params* p) {  // optimizers.hpp:92-135
@@ -294,6 +301,11 @@ int tb200_problem_create(const tb200_problem_desc* d, int device, tb200_problem*
   P->cast_cap = cast_cap;
   std::vector<std::pair<int, int>> cart_ref, coll_ref, vel_ref;  // (list id: 0 cost 1 eq 2 ineq, index)
   bool has_vel = false, has_cast = false, has_discrete = false;
+  // (term, step) that hatched each object of the three lists (tb200_problem_objects)
+  std::vector<std::pair<int, int>> cost_src, eq_src, ineq_src;
+  auto note = [&](const std::vector<DevObj>& lst, int k, int step) {
+    (&lst == &costs ? cost_src : (&lst == &eqs ? eq_src : ineq_src)).push_back({k, step});
+  };
   for (int k = 0; k < d->n_terms; ++k) {
     const tb200_term& tm = d->terms[k];
     if (tm.role != TB200_ROLE_COST && tm.role != TB200_ROLE_CNT) return fail(TB200_ERR_INVALID, "term role must be COST or CNT");
@@ -318,10 +330,12 @@ int tb200_problem_create(const tb200_problem_desc* d, int device, tb200_problem*
         o.kind = zero_tol ? OBJ_JOINT_EQ_COST : OBJ_JOINT_INEQ_COST;
         o.n_rows = zero_tol ? 0 : 2 * o.n_steps * D;
         costs.push_back(o);
+        note(costs, k, tm.first_step);
       } else {
         o.kind = zero_tol ? OBJ_JOINT_EQ_CNT : OBJ_JOINT_INEQ_CNT;
         o.n_rows = (zero_tol ? 1 : 2) * o.n_steps * D;
         (zero_tol ? eqs : ineqs).push_back(o);
+        note(zero_tol ? eqs : ineqs, k, tm.first_step);
       }
       max_rows += o.n_rows;
     } else if (tm.kind == TB200_TERM_CART_POSE) {
@@ -348,6 +362,7 @@ int tb200_problem_create(const tb200_problem_desc* d, int device, tb200_problem*
       max_rows += ct.n_idx;
       if (is_cnt) { cart_ref.push_back({1, static_cast<int>(eqs.size())}); eqs.push_back(o); }
       else { cart_ref.push_back({0, static_cast<int>(costs.size())}); costs.push_back(o); }
+      note(is_cnt ? eqs : costs, k, tm.first_step);
     } else if (tm.kind == TB200_TERM_COLLISION) {
       if (tm.evaluator_type < TB200_COLL_DISCRETE || tm.evaluator_type > TB200_COLL_LVS_CONTINUOUS)
         return fail(TB200_ERR_INVALID, "unknown collision evaluator type");
@@ -381,6 +396,7 @@ int tb200_problem_create(const tb200_problem_desc* d, int device, tb200_problem*
         c.lvs = (tm.evaluator_type == TB200_COLL_CONTINUOUS) ? std::numeric_limits<double>::max() : tm.longest_valid_segment_length;
         if (is_cnt) { coll_ref.push_back({2, static_cast<int>(ineqs.size())}); ineqs.push_back(c); }
         else { coll_ref.push_back({0, static_cast<int>(costs.size())}); costs.push_back(c); }
+        note(is_cnt ? ineqs : costs, k, t);
       }
     } else if (tm.kind == TB200_TERM_CART_VEL) {
       // CartVelTermInfo::hatch (problem_description.cpp:1011-1057): one object per step pair (t, t+1)
@@ -403,6 +419,7 @@ int tb200_problem_create(const tb200_problem_desc* d, int device, tb200_problem*
         has_vel = true;
         if (is_cnt) { vel_ref.push_back({2, static_cast<int>(ineqs.size())}); ineqs.push_back(c); }
         else { vel_ref.push_back({0, static_cast<int>(costs.size())}); costs.push_back(c); }
+        note(is_cnt ? ineqs : costs, k, t);
       }
     } else {
       return fail(TB200_ERR_INVALID, "unknown term kind");
@@ -414,6 +431,9 @@ int tb200_problem_create(const tb200_problem_desc* d, int device, tb200_problem*
         n_coll_cand += o.n_rows;
         max_rows += o.n_rows;
       }
+  P->obj_src = cost_src;
+  P->obj_src.insert(P->obj_src.end(), eq_src.begin(), eq_src.end());
+  P->obj_src.insert(P->obj_src.end(), ineq_src.begin(), ineq_src.end());
   P->cost_objs = costs;
   P->cnt_objs = eqs;
   P->cnt_objs.insert(P->cnt_objs.end(), ineqs.begin(), ineqs.end());
@@ -737,7 +757,7 @@ int tb200_problem_set_inputs(tb200_problem* P, const double* init_traj, const do
 }
 
 namespace {
-__global__ void reset_state_kernel(DevProblem p) {
+__global__ void reset_state_kernel(DevProblem p, int* log_len, int* log_dropped) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b == 0) {
     p.active_count[0] = p.B;
@@ -768,6 +788,10 @@ __global__ void reset_state_kernel(DevProblem p) {
   p.sqp_top[b] = 0;  // (set by the initial evaluation)
   p.ended_by[b] = 0;
   if (b < p.B / p.group_size) p.group_done[b] = 0;
+  if (log_len) {  // (the SQP log is on)
+    log_len[b] = 0;
+    log_dropped[b] = 0;
+  }
 }
 
 struct GroupOut {
@@ -854,6 +878,39 @@ int launchGroupSelect(tb200_problem* P, int G) {
   return TB200_OK;
 }
 
+// Doubles of one SQP log record (DevProblem::log): header, merit coefficients, model values, exact values, point.
+size_t logStride(const tb200_problem* P, int with_x) {
+  const size_t nc = P->dp.n_costs, nk = P->dp.n_cnts;
+  return kLogHeader + 3 * nk + 2 * nc + (with_x ? static_cast<size_t>(P->N) : 0);
+}
+// The log setting of tb200_problem_set_sqp_log takes effect here, at the start of a solve: the record buffer is
+// (re)allocated when its shape changed and released when the log is off.
+int applyLogSetting(tb200_problem* P) {
+  EvalExtra& ex = P->ex;
+  const int cap = P->log_cap_next, wx = P->log_with_x_next;
+  const size_t stride = logStride(P, wx);
+  const bool keep = cap > 0 && ex.log != nullptr && ex.log_cap == cap && ex.log_with_x == wx;
+  // off until the buffers of the new setting exist: a failed allocation leaves the log off, not pointing at freed memory
+  P->log_solved = false;
+  ex.log = nullptr; ex.log_len = ex.log_dropped = nullptr;
+  ex.log_cap = ex.log_stride = ex.log_with_x = 0;
+  if (!keep) {
+    P->log.release(); P->log_len.release(); P->log_dropped.release();
+    if (cap == 0) return TB200_OK;
+    cudaError_t e = P->log.alloc(static_cast<size_t>(P->B) * cap * stride);
+    if (e == cudaSuccess) e = P->log_len.alloc(P->B);
+    if (e == cudaSuccess) e = P->log_dropped.alloc(P->B);
+    if (e != cudaSuccess) {
+      P->log.release(); P->log_len.release(); P->log_dropped.release();
+      return fail(TB200_ERR_CUDA, std::string("SQP log buffer of ") + std::to_string(cap) + " records: " + cudaGetErrorString(e));
+    }
+  }
+  ex.log = P->log.p; ex.log_len = P->log_len.p; ex.log_dropped = P->log_dropped.p;
+  ex.log_cap = cap; ex.log_stride = static_cast<int>(stride); ex.log_with_x = wx;
+  P->log_solved = true;
+  return TB200_OK;
+}
+
 cudaEvent_t getEvent(tb200_problem* P, size_t i) {
   while (P->events.size() <= i) {
     cudaEvent_t e;
@@ -873,9 +930,10 @@ int tb200_solve_batch_resident(tb200_problem* P) {
   const int64_t h2d = tm.h2d_bytes;
   tm = tb200_timing{};
   tm.h2d_bytes = h2d;
+  if (int rc = applyLogSetting(P)) return rc;
   cudaEvent_t e_begin = getEvent(P, 0), e_end = getEvent(P, 1), e_init0 = getEvent(P, 2), e_init1 = getEvent(P, 3);
   CK(cudaEventRecord(e_begin, st));
-  reset_state_kernel<<<(dp.B + 127) / 128, 128, 0, st>>>(dp);
+  reset_state_kernel<<<(dp.B + 127) / 128, 128, 0, st>>>(dp, P->ex.log_len, P->ex.log_dropped);
   if (dp.qp_paths) CK(cudaMemsetAsync(dp.qp_paths, 0, dp.B * sizeof(int), st));
   // the initial evaluation + convexification of every trajectory: one CTA per trajectory (optimizers.cpp:761-783)
   CK(cudaEventRecord(e_init0, st));
@@ -1238,6 +1296,81 @@ int tb200_check_trajectories(tb200_problem* P, const double* x, const tb200_chec
   CK(pull(out->first_slot, a.first_slot, B * sizeof(int)));
   CK(pull(out->min_distance, a.min_distance, B * sizeof(double)));
   CK(cudaStreamSynchronize(st));
+  return TB200_OK;
+}
+
+int tb200_problem_set_sqp_log(tb200_problem* P, int32_t capacity, int32_t with_x) {
+  if (!P) return fail(TB200_ERR_INVALID, "null problem");
+  if (capacity < 0) return fail(TB200_ERR_INVALID, "sqp log capacity must be >= 0 (0: off)");
+  if (with_x != 0 && with_x != 1) return fail(TB200_ERR_INVALID, "with_x must be 0 or 1");
+  // the whole buffer, [batch][capacity][stride] doubles, must be addressable (and its int stride representable)
+  const size_t stride = logStride(P, with_x), limit = std::numeric_limits<size_t>::max() / sizeof(double);
+  if (stride > static_cast<size_t>(INT_MAX) ||
+      (capacity > 0 && static_cast<size_t>(capacity) > limit / stride / static_cast<size_t>(P->B)))
+    return fail(TB200_ERR_INVALID, "sqp log of " + std::to_string(capacity) + " records per trajectory is too large");
+  P->log_cap_next = capacity;
+  P->log_with_x_next = capacity > 0 ? with_x : 0;
+  return TB200_OK;
+}
+
+int tb200_fetch_sqp_log(tb200_problem* P, tb200_sqp_log* out) {
+  if (!P || !out) return fail(TB200_ERR_INVALID, "null argument");
+  if (!P->log_solved) return fail(TB200_ERR_INVALID, "the last solve ran without the SQP log (tb200_problem_set_sqp_log)");
+  const DevProblem& dp = P->dp;
+  const EvalExtra& ex = P->ex;
+  if (out->new_x && !ex.log_with_x) return fail(TB200_ERR_INVALID, "new_x requested, but the log was recorded without x");
+  CK(cudaSetDevice(P->device));
+  const size_t B = dp.B, R = ex.log_cap, S = ex.log_stride, nc = dp.n_costs, nk = dp.n_cnts, N = dp.N;
+  std::vector<double> raw(B * R * S);
+  std::vector<int32_t> len(B), dropped(B);
+  CK(cudaMemcpyAsync(raw.data(), P->log.p, raw.size() * sizeof(double), cudaMemcpyDeviceToHost, P->stream));
+  CK(cudaMemcpyAsync(len.data(), P->log_len.p, B * sizeof(int), cudaMemcpyDeviceToHost, P->stream));
+  CK(cudaMemcpyAsync(dropped.data(), P->log_dropped.p, B * sizeof(int), cudaMemcpyDeviceToHost, P->stream));
+  CK(cudaStreamSynchronize(P->stream));
+  const double qnan = std::numeric_limits<double>::quiet_NaN();
+  for (size_t b = 0; b < B; ++b) {
+    if (out->n_records) out->n_records[b] = len[b];
+    if (out->n_dropped) out->n_dropped[b] = dropped[b];
+    const double* old = nullptr;  // exact values of the last accepted point: the record of kind 0 or the last accept
+    for (size_t r = 0; r < R; ++r) {
+      const size_t i = b * R + r;
+      const bool have = static_cast<int>(r) < len[b];
+      const double* h = raw.data() + i * S;
+      const double* mu = h + kLogHeader;
+      const double *mc = mu + nk, *mk = mc + nc, *vc = mk + nk, *vk = vc + nc, *x = vk + nk;
+      auto put_i = [&](int32_t* dst, int f) { if (dst) dst[i] = have ? static_cast<int32_t>(h[f]) : 0; };
+      auto put_d = [&](double* dst, int f) { if (dst) dst[i] = have ? h[f] : qnan; };
+      auto put_v = [&](double* dst, const double* src, size_t n) {
+        if (dst) for (size_t k = 0; k < n; ++k) dst[i * n + k] = (have && src) ? src[k] : qnan;
+      };
+      put_i(out->kind, LOG_KIND); put_i(out->merit_round, LOG_ROUND); put_i(out->iter, LOG_ITER);
+      put_d(out->trust_box_size, LOG_TRUST);
+      put_d(out->old_merit, LOG_OLD_MERIT); put_d(out->model_merit, LOG_MODEL_MERIT); put_d(out->new_merit, LOG_NEW_MERIT);
+      put_i(out->action, LOG_ACTION); put_i(out->ended, LOG_ENDED);
+      const bool qp = have && h[LOG_KIND] == 1;
+      if (out->qp_status) out->qp_status[i] = qp ? static_cast<int32_t>(h[LOG_QP_STATUS]) : -1;
+      if (out->admm_iters) out->admm_iters[i] = qp ? static_cast<int32_t>(h[LOG_ADMM_ITERS]) : 0;
+      if (out->polish) out->polish[i] = qp ? static_cast<int32_t>(h[LOG_POLISH]) : 0;
+      if (out->qp_diag)
+        for (int k = 0; k < 4; ++k) out->qp_diag[i * 4 + k] = qp ? h[(k < 3 ? LOG_PRI_RES + k : LOG_WARM)] : qnan;
+      put_v(out->merit_coeffs, mu, nk);
+      put_v(out->model_cost_vals, mc, nc); put_v(out->model_cnt_viols, mk, nk);
+      put_v(out->new_cost_vals, vc, nc); put_v(out->new_cnt_viols, vk, nk);
+      put_v(out->old_cost_vals, qp ? old : nullptr, nc);
+      put_v(out->old_cnt_viols, qp ? (old ? old + nc : nullptr) : nullptr, nk);
+      if (out->new_x) put_v(out->new_x, x, N);
+      if (have && (h[LOG_KIND] == 0 || h[LOG_ACTION] == 1)) old = vc;  // (vc, vk are adjacent)
+    }
+  }
+  return TB200_OK;
+}
+
+int tb200_problem_objects(const tb200_problem* P, int32_t* term, int32_t* step) {
+  if (!P) return fail(TB200_ERR_INVALID, "null problem");
+  for (size_t i = 0; i < P->obj_src.size(); ++i) {
+    if (term) term[i] = P->obj_src[i].first;
+    if (step) step[i] = P->obj_src[i].second;
+  }
   return TB200_OK;
 }
 
