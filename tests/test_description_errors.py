@@ -43,6 +43,17 @@ def _set_term(d, k, **kw):
         setattr(d._terms[k], name, v)
 
 
+def _moving_segment(d):
+    return next(s for s in d._segs if s.joint_type != capi.JOINT_FIXED)
+
+
+def _nine_joint_objects():
+    d = problems.config2(B=2, T=10)
+    extra = [problems.joint_term(capi.TERM_JOINT_VEL, capi.ROLE_COST, d.D, 0, d.T - 1) for _ in range(7)]
+    return capi.ProblemDesc(d.robot_spec, d.T, d.terms + extra, d.init_traj, fixed_timesteps=[0],
+                            cart_targets=d.cart_targets, obstacles=d.obstacles)
+
+
 @pytest.mark.parametrize("edit,code,text", [
     (lambda d: setattr(d.c, "n_steps", 0), capi.ERR_INVALID, "n_steps out of range"),
     (lambda d: setattr(d.c, "batch", 0), capi.ERR_INVALID, "batch must be >= 1"),
@@ -54,10 +65,44 @@ def _set_term(d, k, **kw):
     (lambda d: _set_term(d, 0, role=7), capi.ERR_INVALID, "term role must be COST or CNT"),
     (lambda d: _set_term(d, 0, kind=42), capi.ERR_INVALID, "unknown term kind"),
     (lambda d: _set_term(d, 0, last_step=500), capi.ERR_INVALID, "joint term steps outside the trajectory"),
+    (lambda d: setattr(d._segs[1], "parent", 1), capi.ERR_INVALID, "segments must be topologically ordered"),
+    (lambda d: setattr(_moving_segment(d), "q_index", 99), capi.ERR_INVALID, "bad q_index"),
+    (lambda d: setattr(d._spheres[0], "segment", 999), capi.ERR_INVALID, "sphere attached to a bad segment"),
+    (lambda d: setattr(d.c.robot, "n_segments", 0), capi.ERR_INVALID, "n_segments out of range"),
+    (lambda d: setattr(d.c.robot, "n_spheres", 33), capi.ERR_INVALID, "too many collision spheres"),
+    (lambda d: setattr(d.c, "n_obstacles", 0), capi.ERR_INVALID, "collision term needs robot spheres and obstacles"),
+    (lambda d: _set_term(d, 3, last_step=50), capi.ERR_INVALID, "collision step outside the trajectory"),
+    (lambda d: _set_term(d, 2, kind=capi.TERM_CART_VEL, link=99), capi.ERR_INVALID, "cart_vel link out of range"),
+    (lambda d: _set_term(d, 2, kind=capi.TERM_CART_VEL, first_step=0, last_step=9), capi.ERR_INVALID,
+     "cart_vel: step pair beyond the trajectory"),
+    (lambda d: _set_term(d, 2, target_slot=1), capi.ERR_INVALID, "cart_pose target_slot out of range"),
+    (lambda d: _set_term(d, 1, first_step=5, last_step=6), capi.ERR_INVALID, "joint term: trajectory is too short"),
 ])
 def test_bad_descriptions_are_refused_before_the_device(edit, code, text):
     rc, msg = _variant(edit)
     assert rc == code and text in msg, (rc, msg)
+
+
+def test_fixed_dof_outside_the_robot():
+    d = problems.config_variants(B=1, T=10)
+    d._fixed_d[0] = 7
+    rc, msg = _create(d)
+    assert rc == capi.ERR_INVALID and "DOF(aka Joint) indice is greater than the number of DOF available." in msg
+
+
+def test_more_than_eight_joint_objects_are_refused():
+    rc, msg = _create(_nine_joint_objects())
+    assert rc == capi.ERR_UNSUPPORTED and "more than 8 joint-space cost/constraint objects" in msg, (rc, msg)
+
+
+@pytest.mark.parametrize("edit,text", [
+    # the robot is checked before the terms, the terms before the fixed timesteps
+    (lambda d: (setattr(d._spheres[0], "segment", 999), _set_term(d, 3, evaluator_type=9)), "sphere attached to a bad segment"),
+    (lambda d: (d._fixed_t.__setitem__(0, 10), _set_term(d, 0, role=7)), "term role must be COST or CNT"),
+])
+def test_the_first_fault_is_reported(edit, text):
+    rc, msg = _variant(edit)
+    assert rc == capi.ERR_INVALID and text in msg, (rc, msg)
 
 
 def test_fixed_timestep_outside_the_trajectory():

@@ -1,5 +1,6 @@
 // Device-side data model of the batched SQP hot path (sm_90a).  See DESIGN.md §3 for the HBM layout.
 #pragma once
+#include <cstddef>
 #include <cstdint>
 
 namespace tb200 {
@@ -43,12 +44,26 @@ struct DevObj {
   int src_off;    // cart: first row in the cart buffers; collision: first candidate
   int n_rows;     // cart: rows; collision: candidates (n_spheres * n_obstacles); joint: rows emitted
   int link;       // cart: segment
-  int target_slot;
-  int pad0;       // index of the object in its own list (cost / cnt)
-  int pad1;       // cart_vel: joints moving the link (bit mask); cast collision: bit 0 start fixed, bit 1 end fixed, bit 2 LVS_DISCRETE
+  union {
+    int target_slot;  // cart_pose: static target in cart_targets[b] (-1: the term's own target_pose)
+    int kernel_slot;  // collision: position in the kernel order (coll_objs), where the evaluation kernel leaves its value
+  };
+  int list_index;  // cart, vel and coll tables: index of the object in cost_objs (cost) or cnt_objs (constraint)
+  union {
+    int joint_mask;  // cart_vel: joints moving the link (bit mask)
+    int cast_flags;  // cast collision: CAST_START_FIXED, CAST_END_FIXED, CAST_LVS_DISCRETE
+  };
   double coeff, margin, buffer;
-  double lvs;     // cast collision: longest valid segment length (max double: never subdivide); cart_vel: max_displacement
+  // cast collision: longest valid segment length (max double: never subdivide); cart_vel: max_displacement.  (One
+  // name: unlike the int unions above, a union of the two doubles changes the evaluation kernel's instructions.)
+  double lvs;
 };
+enum CastFlag { CAST_START_FIXED = 1, CAST_END_FIXED = 2, CAST_LVS_DISCRETE = 4 };  // DevObj::cast_flags
+// the evaluation kernel copies the collision objects to shared memory as raw doubles
+static_assert(sizeof(DevObj) == 80, "DevObj layout");
+static_assert(offsetof(DevObj, coeff) == 48 && offsetof(DevObj, margin) == 56 && offsetof(DevObj, buffer) == 64 &&
+                  offsetof(DevObj, lvs) == 72,
+              "DevObj layout");
 struct DevJointTerm {
   double coeffs[kMaxDof], targets[kMaxDof], upper[kMaxDof], lower[kMaxDof];
 };

@@ -81,7 +81,7 @@ struct EvalExtra {
   const DevObj* vel_objs;            // CartVel step pairs
   int joint_seg[kMaxDof];            // segment that carries trajectory column j
   int joint_obj_idx[8];  // positions of the joint-space objects in the (costs, cnts) list
-  const DevObj* cart_objs;   // pad0 = index in its own list (cost / cnt), is_cnt says which list
+  const DevObj* cart_objs;   // list_index = index in its own list (cost / cnt), is_cnt says which list
   const DevObj* coll_objs;
   int qtype[kMaxDof];                // joint type per trajectory column
   unsigned sphere_jmask[kMaxSpheres];  // which columns move each sphere
@@ -522,12 +522,12 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
       double* jac_out = p.cart_jac + (slot * p.n_cart_rows + o.src_off) * p.cart_stride;
       if (e < 6) {
         const int i = e % 3;
-        err_out[e] = (e < 3) ? p1[i] - p0[i] - o.lvs : p0[i] - p1[i] - o.lvs;
+        err_out[e] = (e < 3) ? p1[i] - p0[i] - o.lvs : p0[i] - p1[i] - o.lvs;  // (lvs: max_displacement)
       } else {
         const int col = e - 6, k = col / D, j = col % D;
         const double* ab = sm + S.jax + ((o.first + k) * D + j) * 6;
         const double* pk = k ? p1 : p0;
-        const bool moves = (o.pad1 >> j) & 1;
+        const bool moves = (o.joint_mask >> j) & 1;
         const double J[3] = {ab[1] * pk[2] - ab[2] * pk[1] - ab[3], ab[2] * pk[0] - ab[0] * pk[2] - ab[4],
                              ab[0] * pk[1] - ab[1] * pk[0] - ab[5]};
         for (int i = 0; i < 3; ++i) {
@@ -682,7 +682,7 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
         // LVS_DISCRETE (DiscreteCollisionEvaluator, collision_terms.cpp:744-893): the same machinery with a discrete test
         // at each of the nsub + 1 STATES of the sub-trajectory (a sub-segment of zero length: s = 0, cc_time = i / nsub,
         // Time0 | Time1 at the waypoints, one link frame for both reference points).
-        const bool sfix = co.pad1 & 1, efix = co.pad1 & 2, disc = co.pad1 & 4;
+        const bool sfix = co.cast_flags & CAST_START_FIXED, efix = co.cast_flags & CAST_END_FIXED, disc = co.cast_flags & CAST_LVS_DISCRETE;
         const double* q0 = xs + t * D;
         const double* q1 = q0 + D;
         double d2 = 0.0;
@@ -890,7 +890,7 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
         const double* e = p.cart_err + slot * p.n_cart_rows + o.src_off;
         for (int r = 0; r < 6; ++r) v += is_cnt ? fmax(e[r], 0.0) : fabs(e[r]);  // INEQ violation | ABS cost
       } else {
-        v = sm[S.objv + o.target_slot];  // collision object: summed by the warp that built its rows
+        v = sm[S.objv + o.kernel_slot];  // collision object: summed by the warp that built its rows
       }
       if (is_cnt) out_viol[i - p.n_costs] = v;
       else out_cost[i] = v;

@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "../../include/trajopt_b200.h"
+#include "dev_buf.h"
 
 namespace {
 constexpr int kThreads = 256;
@@ -554,49 +555,37 @@ int tb200_qp_solve_general(const tb200_qp_general* qp, const tb200_qp_settings* 
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
     return fail(TB200_ERR_NO_DEVICE, "no CUDA device: trajopt_b200 has no CPU fallback");
   if (device < 0 || device >= ndev) return fail(TB200_ERR_INVALID, "bad device ordinal");
-#define GCK(call)                                                                                  \
-  do {                                                                                             \
-    cudaError_t e_ = (call);                                                                       \
-    if (e_ != cudaSuccess) return fail(TB200_ERR_CUDA, std::string(#call) + ": " + cudaGetErrorString(e_)); \
-  } while (0)
-  GCK(cudaSetDevice(device));
+  CK(cudaSetDevice(device));
   tb200_qp_settings st;
   if (settings) st = *settings;
   else tb200_default_qp_settings(&st);
   const size_t nn = static_cast<size_t>(n) * n, mn = static_cast<size_t>(m) * n;
   const size_t ws = 2 * (nn + 2) + (mn + 2) + 14 * (static_cast<size_t>(n) + 2) + 16 * (static_cast<size_t>(m) + 2);
-  double *dP = nullptr, *dq = nullptr, *dA = nullptr, *dl = nullptr, *du = nullptr, *dws = nullptr, *dx = nullptr, *dy = nullptr;
-  int* dint = nullptr;
-  auto release = [&]() {
-    cudaFree(dP); cudaFree(dq); cudaFree(dA); cudaFree(dl); cudaFree(du); cudaFree(dws); cudaFree(dx); cudaFree(dy); cudaFree(dint);
-  };
+  tb200::DevBuf<double> dP, dq, dA, dl, du, dws, dx, dy;
+  tb200::DevBuf<int> dint;
   cudaError_t e = cudaSuccess;
-  auto alloc = [&](double** p, size_t cnt) {
-    if (e == cudaSuccess) e = cudaMalloc(p, std::max<size_t>(cnt, 1) * sizeof(double));
+  auto alloc = [&](auto& buf, size_t cnt) {
+    if (e == cudaSuccess) e = buf.alloc(cnt);
   };
-  alloc(&dP, B * nn); alloc(&dq, static_cast<size_t>(B) * n); alloc(&dA, B * mn); alloc(&dl, static_cast<size_t>(B) * m);
-  alloc(&du, static_cast<size_t>(B) * m); alloc(&dws, B * ws); alloc(&dx, static_cast<size_t>(B) * n); alloc(&dy, static_cast<size_t>(B) * std::max(m, 1));
-  if (e == cudaSuccess) e = cudaMalloc(&dint, 3 * static_cast<size_t>(B) * sizeof(int));
-  if (e != cudaSuccess) {
-    release();
-    return fail(TB200_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e));
-  }
-  auto up = [&](double* d, const double* h, size_t cnt) {
-    if (e == cudaSuccess && cnt) e = cudaMemcpy(d, h, cnt * sizeof(double), cudaMemcpyHostToDevice);
+  alloc(dP, B * nn); alloc(dq, static_cast<size_t>(B) * n); alloc(dA, B * mn); alloc(dl, static_cast<size_t>(B) * m);
+  alloc(du, static_cast<size_t>(B) * m); alloc(dws, B * ws); alloc(dx, static_cast<size_t>(B) * n); alloc(dy, static_cast<size_t>(B) * std::max(m, 1));
+  alloc(dint, 3 * static_cast<size_t>(B));
+  if (e != cudaSuccess) return fail(TB200_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e));
+  auto up = [&](tb200::DevBuf<double>& d, const double* h, size_t cnt) {
+    if (e == cudaSuccess && cnt) e = cudaMemcpy(d.p, h, cnt * sizeof(double), cudaMemcpyHostToDevice);
   };
   up(dP, qp->P, B * nn); up(dq, qp->q, static_cast<size_t>(B) * n); up(dA, qp->A, B * mn); up(dl, qp->l, static_cast<size_t>(B) * m);
   up(du, qp->u, static_cast<size_t>(B) * m);
   if (e == cudaSuccess) {
-    GqDev g{n, m, B, dP, dq, dA, dl, du, dws, ws, st, dx, dy, dint, dint + B, dint + 2 * B};
+    GqDev g{n, m, B, dP.p, dq.p, dA.p, dl.p, du.p, dws.p, ws, st, dx.p, dy.p, dint.p, dint.p + B, dint.p + 2 * B};
     general_qp_kernel<<<B, kThreads>>>(g);
     e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
   }
   std::vector<int> hint(3 * static_cast<size_t>(B));
-  if (e == cudaSuccess) e = cudaMemcpy(x, dx, static_cast<size_t>(B) * n * sizeof(double), cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess && y && m > 0) e = cudaMemcpy(y, dy, static_cast<size_t>(B) * m * sizeof(double), cudaMemcpyDeviceToHost);
-  if (e == cudaSuccess) e = cudaMemcpy(hint.data(), dint, hint.size() * sizeof(int), cudaMemcpyDeviceToHost);
-  release();
+  if (e == cudaSuccess) e = cudaMemcpy(x, dx.p, static_cast<size_t>(B) * n * sizeof(double), cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess && y && m > 0) e = cudaMemcpy(y, dy.p, static_cast<size_t>(B) * m * sizeof(double), cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess) e = cudaMemcpy(hint.data(), dint.p, hint.size() * sizeof(int), cudaMemcpyDeviceToHost);
   if (e != cudaSuccess) return fail(TB200_ERR_CUDA, std::string("general QP: ") + cudaGetErrorString(e));
   for (int b = 0; b < B; ++b) {
     status[b] = hint[b];
@@ -604,7 +593,6 @@ int tb200_qp_solve_general(const tb200_qp_general* qp, const tb200_qp_settings* 
     if (polish) polish[b] = hint[2 * B + b];
   }
   return TB200_OK;
-#undef GCK
 }
 
 }  // extern "C"
