@@ -43,10 +43,14 @@ static __device__ unsigned long long g_prof[32];
 #define PROF_T0() const long long prof_t0_ = clock64()
 #define PROF_ADD(slot) do { if (q.tid == 0) atomicAdd(&g_prof[slot], (unsigned long long)(clock64() - prof_t0_)); } while (0)
 #define PROF_COUNT(slot) do { if (q.tid == 0) atomicAdd(&g_prof[slot], 1ull); } while (0)
+// the same cycles into two slots (a total and its share of one kind)
+#define PROF_ADD2(slot, slot2) do { if (q.tid == 0) { const unsigned long long d_ = clock64() - prof_t0_; \
+    atomicAdd(&g_prof[slot], d_); atomicAdd(&g_prof[slot2], d_); } } while (0)
 #else
 #define PROF_T0()
 #define PROF_ADD(slot)
 #define PROF_COUNT(slot)
+#define PROF_ADD2(slot, slot2)
 #endif
 // -DTB200_PROFILE_CHECK: the per-level slots of the solve (4, 14, 15, 9) count the parts of a termination check instead
 #if defined(TB200_PROFILE) && defined(TB200_PROFILE_CHECK)
@@ -245,7 +249,8 @@ struct QpCtx {
   double* scratch;
   int pinv;              // the ADMM system is factored in its partition-inverse form (pl)
   PinvPlan pl;
-  double* pi_g;          // this CTA's block of global memory for the rows of the partition inverses [PR][3 NB]
+  double* pi_g;          // this CTA's block of global memory for the rows of the partition inverses, column-major
+                         // [3 NB][PR]: a warp's loads and stores of one column are contiguous
   double* z_stash;       // ... and for the copy of Z taken before a polish
   double c, cinv, rho, rho_eq, sigma, alpha;
   __device__ __forceinline__ double* R(int r) const { return rows + static_cast<size_t>(r) * RS; }
@@ -308,6 +313,9 @@ __device__ __forceinline__ void block_reduce(const QpCtx& q, double (&vals)[NQ])
 struct SysW {
   bool polish;
   double sig, rho_aux;
+#ifdef TB200_PROFILE
+  int prof_kind = 0;  // the profiler slots of assemble_factor: 0 the initial factorisation, 1 a later one (polish: 2)
+#endif
 };
 
 // variable index of coefficient k of a row (padding coefficients alias the last real one; their value is 0)
@@ -363,28 +371,39 @@ __device__ __forceinline__ void row_times_matT(double (&out)[NB], const double (
     out[j] += a0 + a1;
   }
 }
-template <int NB>
+// WARP (blocks of <= 16 with the factor in shared memory): every block is inverted by one half warp, lanes 0..NB-1 of
+// the half holding its rows, so the steps of an inversion synchronise that warp only; the factor is addressed as
+// shared memory.  Otherwise the blocks of a chunk lie side by side over the CTA and every step is a CTA barrier.  Both
+// compute every value by the same expression in the same order.
+template <int NB, bool WARP>
 __device__ inline bool bcr_factor(const QpCtx& q) {
+  static_assert(!WARP || NB <= 16, "a block per half warp");
   constexpr int BLK = NB * NB, G = kQpThreads / 2;  // two thread groups work side by side where possible
-  constexpr int CH1 = kQpThreads / NB, CH2 = G / NB;  // blocks per task chunk: inversion (all threads) / products (per group)
+  // blocks per task chunk: inversion (all threads) / products (per group)
+  constexpr int CH1 = WARP ? kQpThreads / 16 : kQpThreads / NB, CH2 = G / NB;
+  extern __shared__ double sm[];
+  double* const SA = WARP ? sm + (q.SA - q.smbase) : q.SA;
+  double* const SLM = WARP ? sm + (q.SLM - q.smbase) : q.SLM;
+  double* const SU = WARP ? sm + (q.SU - q.smbase) : q.SU;
   const int M = q.M, tid = q.tid;
   const int grp = tid >= G, gt = tid - (grp ? G : 0);
   int bad = 0;
   for (int l = 0; (1 << l) - 1 < M; ++l) {
     const int s = 1 << l, first = s - 1, sh = l + 1;  // eliminated p = first + (e << sh); survivors j = p + s
     const int nE = (M + s) >> sh, nS = M >> sh;
+    PROF_T0();
     // ---- 1. Ainv_p in place: Gauss-Jordan without pivoting (the blocks are symmetric positive definite);
     //         thread (e,i) keeps row i of block e in registers, the pivot row goes through shared memory
     for (int e0 = 0; e0 < nE; e0 += CH1) {
       const int nc = (nE - e0 < CH1) ? nE - e0 : CH1;
-      const bool act = tid < nc * NB;
-      const int e = act ? tid / NB : 0, i = tid % NB;
-      double* A = q.SA + (first + ((e0 + e) << sh)) * BLK + i * NB;
+      const int e = WARP ? tid >> 4 : tid / NB, i = WARP ? tid & 15 : tid % NB;
+      const bool act = WARP ? (i < NB && e < nc) : tid < nc * NB;
+      double* A = SA + (first + ((e0 + (act ? e : 0)) << sh)) * BLK + (act ? i : 0) * NB;
       double a[NB];
       load_row<NB>(a, A);
 #pragma unroll
       for (int k = 0; k < NB; ++k) {
-        double* prow = q.tmp + (k & 1) * (CH1 * NB) + e * NB;
+        double* prow = q.tmp + (k & 1) * (CH1 * NB) + e * NB;  // (double buffered: one barrier per step)
         if (act && i == k) {
           const double piv = a[k];
           if (!(piv > 0.0)) bad = 1;
@@ -393,7 +412,8 @@ __device__ inline bool bcr_factor(const QpCtx& q) {
           for (int j = 0; j < NB; ++j) a[j] = (j == k) ? ip : a[j] * ip;
           store_row<NB>(prow, a);
         }
-        __syncthreads();
+        if constexpr (WARP) __syncwarp();
+        else __syncthreads();
         if (act && i != k) {
           double pr[NB];
           load_row<NB>(pr, prow);
@@ -405,30 +425,31 @@ __device__ inline bool bcr_factor(const QpCtx& q) {
       if (act) store_row<NB>(A, a);
     }
     __syncthreads();
+    PROF_ADD(30);  // (the inversions of every level, all factorisations by the cyclic reduction)
     // ---- 2. group 0: Up_p = L_{p+s} Ainv_p -> SU[p];  group 1: Um_p = L_p' Ainv_p -> SU[p-s] (temporary home)
     for (int e0 = 0; e0 < nE; e0 += CH2) {
       const int nc = (nE - e0 < CH2) ? nE - e0 : CH2;
       const bool act = gt < nc * NB;
       const int e = e0 + (act ? gt / NB : 0), i = gt % NB;
       const int p = first + (e << sh);
-      const double* Ai = q.SA + p * BLK;
+      const double* Ai = SA + p * BLK;
       if (act && grp == 0 && p + s < M) {
         double x[NB], out[NB];
-        load_row<NB>(x, q.SLM + (p + s) * BLK + i * NB);
+        load_row<NB>(x, SLM + (p + s) * BLK + i * NB);
 #pragma unroll
         for (int j = 0; j < NB; ++j) out[j] = 0.0;
         row_times_mat<NB>(out, x, Ai);
-        store_row<NB>(q.SU + p * BLK + i * NB, out);
+        store_row<NB>(SU + p * BLK + i * NB, out);
       }
       if (act && grp == 1 && p - s >= 0) {
         double x[NB], out[NB];
-        const double* L = q.SLM + p * BLK + i;  // column i of L_p
+        const double* L = SLM + p * BLK + i;  // column i of L_p
 #pragma unroll
         for (int k = 0; k < NB; ++k) x[k] = L[k * NB];
 #pragma unroll
         for (int j = 0; j < NB; ++j) out[j] = 0.0;
         row_times_mat<NB>(out, x, Ai);
-        store_row<NB>(q.SU + (p - s) * BLK + i * NB, out);
+        store_row<NB>(SU + (p - s) * BLK + i * NB, out);
       }
     }
     __syncthreads();
@@ -445,34 +466,34 @@ __device__ inline bool bcr_factor(const QpCtx& q) {
       for (int c = 0; c < NB; ++c) keep[c] = 0.0;
       if (act && grp == 0) {
         double x[NB], t1[NB];
-        load_row<NB>(x, q.SU + p * BLK + i * NB);  // row i of Up_p
+        load_row<NB>(x, SU + p * BLK + i * NB);  // row i of Up_p
 #pragma unroll
         for (int c = 0; c < NB; ++c) t1[c] = 0.0;
-        row_times_matT<NB>(t1, x, q.SLM + j * BLK);
-        if (p - s >= 0) row_times_mat<NB>(keep, x, q.SLM + p * BLK);
+        row_times_matT<NB>(t1, x, SLM + j * BLK);
+        if (p - s >= 0) row_times_mat<NB>(keep, x, SLM + p * BLK);
         double arow[NB];
-        load_row<NB>(arow, q.SA + j * BLK + i * NB);
+        load_row<NB>(arow, SA + j * BLK + i * NB);
 #pragma unroll
         for (int c = 0; c < NB; ++c) arow[c] -= t1[c];
-        store_row<NB>(q.SA + j * BLK + i * NB, arow);
+        store_row<NB>(SA + j * BLK + i * NB, arow);
       }
       if (act && grp == 1 && j + s < M) {
         double x[NB];
-        load_row<NB>(x, q.SU + j * BLK + i * NB);  // row i of Um_{j+s}
-        row_times_mat<NB>(keep, x, q.SLM + (j + s) * BLK);
+        load_row<NB>(x, SU + j * BLK + i * NB);  // row i of Um_{j+s}
+        row_times_mat<NB>(keep, x, SLM + (j + s) * BLK);
       }
       __syncthreads();
       if (act && grp == 0) {
 #pragma unroll
         for (int c = 0; c < NB; ++c) keep[c] = -keep[c];
-        store_row<NB>(q.SLM + j * BLK + i * NB, keep);  // new left coupling (0 without a left survivor)
+        store_row<NB>(SLM + j * BLK + i * NB, keep);  // new left coupling (0 without a left survivor)
       }
       if (act && grp == 1 && j + s < M) {
         double arow[NB];
-        load_row<NB>(arow, q.SA + j * BLK + i * NB);
+        load_row<NB>(arow, SA + j * BLK + i * NB);
 #pragma unroll
         for (int c = 0; c < NB; ++c) arow[c] -= keep[c];
-        store_row<NB>(q.SA + j * BLK + i * NB, arow);
+        store_row<NB>(SA + j * BLK + i * NB, arow);
       }
     }
     __syncthreads();
@@ -480,7 +501,7 @@ __device__ inline bool bcr_factor(const QpCtx& q) {
     for (int t = tid; t < nE * BLK; t += kQpThreads) {
       const int e = t / BLK, r = t % BLK;
       const int p = first + (e << sh);
-      if (p - s >= 0) q.SLM[p * BLK + r] = q.SU[(p - s) * BLK + r];
+      if (p - s >= 0) SLM[p * BLK + r] = SU[(p - s) * BLK + r];
     }
     __syncthreads();
   }
@@ -1085,8 +1106,10 @@ __device__ __forceinline__ double xbound_weight(const QpCtx& q, const SysW& w, i
 //    not-yet-eliminated rows' diagonal entries do, together with their reciprocal, ready for the row's own pivot step).
 // One pass at the end applies the scales.  scripts/probes/pinv_proto.py holds the same algorithm in numpy (error 1e-15
 // at condition 1e16; a shortcut that published pivot + 1 to get -g by cancellation lost eps * pivot).
-// tmp: [2][nmat][QN + 2] then [nmat][QN] column scales.  Every thread of the CTA calls it (one block barrier per step,
-// n_max steps); returns true when this thread met a non-positive pivot.
+// tmp: [2][nmat][QN + 2] then [nmat][QN] column scales.  Called by the 64 threads of the two warps that hold every row
+// of matrix `mat`: one named barrier (`bar.sync bar, 64`) per step, n_max steps.  (Named barriers 1 and 2 also serve
+// eval_step, which a CTA never runs while it is in a QP step: solve_kernel separates the two by CTA barriers.)  Returns
+// true when this thread met a non-positive pivot.
 // 1 / x for the pivots: hardware seed (about 20 bits) and three Newton steps, straight-line code (the library division
 // keeps a slow-path CALL, and a call inside the elimination loop spills the row around it)
 __device__ __forceinline__ double pivot_rcp(const double x) {
@@ -1101,7 +1124,7 @@ __device__ __forceinline__ double pivot_rcp(const double x) {
 }
 template <int QN>
 __device__ __forceinline__ bool gj_rows(double (&a)[QN], double diag, const bool active, const int mat, const int row,
-                                        const int n, const int n_max, double* tmp, const int nmat) {
+                                        const int n, const int n_max, double* tmp, const int nmat, const int bar) {
   constexpr int BS = QN + 2;  // row + reciprocal (+ pad)
   double* const csv = tmp + 2 * nmat * BS + mat * QN;  // this matrix's column scales
   bool bad = false;
@@ -1123,7 +1146,7 @@ __device__ __forceinline__ bool gj_rows(double (&a)[QN], double diag, const bool
       inv_rs = diag;
       diag = pv_mine;
     }
-    __syncthreads();
+    asm volatile("bar.sync %0, 64;" ::"r"(bar) : "memory");
     if (active && k < n && !piv) {
       const double tr = buf[row];
       const bool ahead = row > k;  // this row is still to be eliminated
@@ -1153,6 +1176,7 @@ template <int NB>
 __device__ inline bool pinv_factor(const QpCtx& q) {
   constexpr int QN = 3 * NB, blk = NB * NB;
   static_assert(QN % 2 == 0, "pivot rows move as double2");
+  static_assert(QN <= 64, "a partition on two warps");
   extern __shared__ double sm[];
   const int tid = q.tid, M = q.M, Np = q.Np;
   const int PR = q.pl.PR, nS = q.pl.nS, Ns = q.pl.Ns, ZS = q.pl.ZS, WS = q.pl.WS, SS = q.pl.SS;
@@ -1172,10 +1196,12 @@ __device__ inline bool pinv_factor(const QpCtx& q) {
 #define PROF_PF(slot)
 #endif
   {
-    // ---- 1. inverse of every partition (the tridiagonal run of <= 3 blocks starting at block 4 p)
-    const bool prow = tid < PR;
-    const int p = prow ? tid / QN : 0, lr = prow ? tid % QN : 0;
-    const int npb = (M - 4 * p) < 3 ? (M - 4 * p) : 3;
+    // ---- 1. inverse of every partition (the tridiagonal run of <= 3 blocks starting at block 4 p): partition p on warps
+    // 2p and 2p + 1, its rows on their first lanes; row lr of partition p is row pr = p QN + lr of PI and W
+    const int p = tid >> 6, lr = tid & 63, pr = p * QN + lr;
+    const bool part = p < nparts;
+    const int npb = !part ? 0 : (M - 4 * p) < 3 ? (M - 4 * p) : 3;
+    const bool prow = lr < npb * NB;
     const int kb = lr / NB, r = lr % NB, gb = 4 * p + kb;  // local block, row inside it, global block
     double a[QN];
 #pragma unroll
@@ -1191,11 +1217,11 @@ __device__ inline bool pinv_factor(const QpCtx& q) {
     }
     PROF_PF(0);
     const double dg = prow ? SA[gb * blk + r * NB + r] : 1.0;  // the row's diagonal entry
-    bad |= gj_rows<QN>(a, dg, prow, p, lr, npb * NB, (M < 3 ? M : 3) * NB, tmp, nparts);
+    if (part) bad |= gj_rows<QN>(a, dg, prow, p, lr, npb * NB, (M < 3 ? M : 3) * NB, tmp, nparts, 1 + p);
     PROF_PF(4);
     if (prow) {
 #pragma unroll
-      for (int j = 0; j < QN; ++j) q.pi_g[tid * QN + j] = a[j];
+      for (int j = 0; j < QN; ++j) q.pi_g[j * PR + pr] = a[j];
       // ---- 2. W = PI C: the left separator couples to the partition's first block (C = SLM[4p]), the right one to its
       // last block (C = SLM[4p + 3]'); a partition that has a right separator is always full (3 blocks)
       const bool has_l = p > 0, has_r = 4 * p + 3 < M;
@@ -1210,8 +1236,8 @@ __device__ inline bool pinv_factor(const QpCtx& q) {
 #pragma unroll
           for (int c = 0; c < NB; ++c) wr += a[2 * NB + c] * SLM[(4 * p + 3) * blk + j * NB + c];
         }
-        W[tid * WS + j] = wl;
-        W[tid * WS + NB + j] = wr;
+        W[pr * WS + j] = wl;
+        W[pr * WS + NB + j] = wr;
       }
     }
   }
@@ -1258,7 +1284,7 @@ __device__ inline bool pinv_factor(const QpCtx& q) {
 #pragma unroll
     for (int j = 0; j < QN; ++j) a[j] = (srow && j < nS) ? S[tid * SS + j] : 0.0;
     const double dg = srow ? S[tid * SS + tid] : 1.0;
-    bad |= gj_rows<QN>(a, dg, srow, 0, tid, nS, nS, tmp, 1);
+    if (tid < 64) bad |= gj_rows<QN>(a, dg, srow, 0, tid, nS, nS, tmp, 1, 1);  // (nS <= 3 NB rows: warps 0 and 1)
     if (srow) {
 #pragma unroll
       for (int j = 0; j < QN; ++j)
@@ -1302,29 +1328,38 @@ __device__ inline bool pinv_factor(const QpCtx& q) {
   return ok;
 }
 
-template <int NB, bool PINV>
+// PINV: the partition-inverse form (pinv_factor), else the cyclic reduction (bcr_factor<NB, WARP>)
+template <int NB, bool PINV, bool WARP>
 __device__ __noinline__ bool assemble_factor(const QpCtx& q, const SysW& w) {
   PROF_T0();
   rows_prepare_weights(q, w);
   constexpr int nb = NB, blk = NB * NB;
+  // (both forms that run on chip address the factor as shared memory; the global-memory factor and the CTA-wide
+  // reference keep generic pointers)
+  extern __shared__ double sm[];
+  constexpr bool SMEM = PINV || WARP;
+  double* const SA = SMEM ? sm + (q.SA - q.smbase) : q.SA;
+  double* const SLM = SMEM ? sm + (q.SLM - q.smbase) : q.SLM;
   const int N = q.N, HB = 2 * q.D, PW = HB + 1, CN = q.CN;
   for (int t = q.tid; t < q.M * blk; t += kQpThreads) {
-    q.SA[t] = 0.0;
-    q.SLM[t] = 0.0;
+    SA[t] = 0.0;
+    SLM[t] = 0.0;
   }
   __syncthreads();
   for (int i = q.tid; i < q.Np; i += kQpThreads) {
     const int p = i / nb, r = i % nb;
-    double* Arow = q.SA + static_cast<size_t>(p) * blk + r * nb;   // K(i, p*nb + c)
-    double* Lrow = q.SLM + static_cast<size_t>(p) * blk + r * nb;   // K(i, (p-1)*nb + c)
+    double* Arow = SA + static_cast<size_t>(p) * blk + r * nb;   // K(i, p*nb + c)
+    double* Lrow = SLM + static_cast<size_t>(p) * blk + r * nb;   // K(i, (p-1)*nb + c)
     if (i >= N) {
       Arow[r] = 1.0;  // padding variable
       continue;
     }
-    // element K(i, i-k), k = 0..HB, lands in the diagonal block (k <= r) or the left coupling block
+    // element K(i, i-k), k = 0..HB, lands in the diagonal block (k <= r) or the left coupling block.  (__dadd_rn: the
+    // sum is never contracted with the product that forms val, whatever the addressing lets the compiler schedule, so
+    // that every factor form assembles the same bits)
     auto add = [&](int k, double val) {
-      if (k <= r) Arow[r - k] += val;
-      else Lrow[nb + r - k] += val;
+      if (k <= r) Arow[r - k] = __dadd_rn(Arow[r - k], val);
+      else Lrow[nb + r - k] = __dadd_rn(Lrow[nb + r - k], val);
     };
     for (int t = 0; t < q.n_band; ++t) {
       const int k = q.band_offs[t];
@@ -1346,16 +1381,21 @@ __device__ __noinline__ bool assemble_factor(const QpCtx& q, const SysW& w) {
   // mirror the strictly lower part of every diagonal block into its upper part
   for (int t = q.tid; t < q.M * blk; t += kQpThreads) {
     const int p = t / blk, i = (t % blk) / nb, j = t % nb;
-    if (j > i) q.SA[static_cast<size_t>(p) * blk + i * nb + j] = q.SA[static_cast<size_t>(p) * blk + j * nb + i];
+    if (j > i) SA[static_cast<size_t>(p) * blk + i * nb + j] = SA[static_cast<size_t>(p) * blk + j * nb + i];
   }
   __syncthreads();
-  PROF_ADD(10);
+  // slots 24 + 2 kind (assembly) and 25 + 2 kind (elimination); kind: 0 initial, 1 rho update or recovery, 2 polish
+#ifdef TB200_PROFILE
+  const int pk = w.polish ? 2 : w.prof_kind;
+  if (pk == 1) PROF_COUNT(31);
+#endif
+  PROF_ADD2(10, 24 + 2 * pk);
   bool ok;
   {
     PROF_T0();
     if constexpr (PINV) ok = pinv_factor<NB>(q);
-    else ok = bcr_factor<NB>(q);
-    PROF_ADD(11);
+    else ok = bcr_factor<NB, WARP>(q);
+    PROF_ADD2(11, 25 + 2 * pk);
   }
   return ok;
 }
@@ -1848,7 +1888,7 @@ __device__ __noinline__ void admm_block_pinv(const QpCtx& q, const double rho_au
     // ================= warps 0-5: partition rows (PI row in registers), separator halves, variables
     double pi[QN];
 #pragma unroll
-    for (int j = 0; j < QN; ++j) pi[j] = prow ? q.pi_g[tid * QN + j] : 0.0;
+    for (int j = 0; j < QN; ++j) pi[j] = prow ? q.pi_g[j * PR + tid] : 0.0;
     bar();  // (the entry pass of the row warps)
 #ifdef TB200_PROFILE
     if (tid == 0) atomicAdd(&g_prof[21], (unsigned long long)(clock64() - prof_entry_));
@@ -2517,17 +2557,19 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
     fn(q, sysw.rho_aux, n, keep_last ? 1 : 0);
   };
   // the same for the factorisation (a few calls per QP, tens of thousands of cycles each); the polish system always
-  // takes the cyclic reduction (its solves are the generic ones)
+  // takes the cyclic reduction (its solves are the generic ones), with warp-local block inversions when the factor is
+  // in shared memory (the CTA-wide ones, same values, under TB200_GENERIC_QP_PASSES=1: the reference of the tests)
   using FactorFn = bool (*)(const QpCtx&, const SysW&);
   auto factorize = [&](const SysW& wts) -> bool {
     fused_chk = false;
-    if constexpr (REGOK) {
-      if (use_pinv && !wts.polish) {
-        FactorFn volatile fn = &assemble_factor<NB, true>;
-        return fn(q, wts);
-      }
+    FactorFn f = &assemble_factor<NB, false, false>;
+    if constexpr (NB <= 16) {
+      if (fast_passes && __isShared(q.SA)) f = &assemble_factor<NB, false, true>;
     }
-    FactorFn volatile fn = &assemble_factor<NB, false>;
+    if constexpr (REGOK) {
+      if (use_pinv && !wts.polish) f = &assemble_factor<NB, true, false>;
+    }
+    FactorFn volatile fn = f;
     return fn(q, wts);
   };
   // A polish factors its own system over Z (the rest of the partition-inverse form lies beyond the cyclic-reduction
@@ -2545,6 +2587,9 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
     if (restore) rows_prepare_weights(q, sysw);
   };
   { PROF_T0(); factor_ok = factorize(sysw); PROF_ADD(6); }
+#ifdef TB200_PROFILE
+  sysw.prof_kind = 1;  // every later factorisation of the ADMM system: a rho update or the recovery after a failed polish
+#endif
 
   double* dxs = q.scratch;              // [Np] last trajectory step (written on check iterations)
   double* dyb = q.scratch + q.Np;       // [Np] last dual step of the variable-bound rows
