@@ -102,7 +102,8 @@ enum {
   TB200_TERM_JOINT_ACC = 2,  /* JointAccTermInfo  -> trajectory_costs.cpp:502-754  */
   TB200_TERM_CART_POSE = 3,  /* CartPoseTermInfo  -> kinematic_terms.cpp:187-366   */
   TB200_TERM_CART_VEL = 4,   /* CartVelTermInfo   -> kinematic_terms.cpp:368-425   */
-  TB200_TERM_COLLISION = 5   /* CollisionTermInfo -> collision_terms.cpp            */
+  TB200_TERM_COLLISION = 5,  /* CollisionTermInfo -> collision_terms.cpp            */
+  TB200_TERM_AVOID_SINGULARITY = 6 /* AvoidSingularityTermInfo -> kinematic_terms.cpp:586-642 */
 };
 enum { TB200_ROLE_COST = 1, TB200_ROLE_CNT = 2 }; /* TermType::TT_COST / TT_CNT */
 
@@ -136,6 +137,12 @@ typedef struct tb200_term {
   double coeff;
   double margin_buffer;     /* collision_margin_buffer: rows are emitted out to margin+buffer */
   double longest_valid_segment_length;
+  /* AVOID_SINGULARITY: one object per step in [first_step, last_step] on the geometric Jacobian of `link` (all
+   * n_dof columns); error 1/(s + lambda) - 1/(0.1 + lambda) with s the smallest singular value, scaled by coeffs[0]
+   * (1: unscaled).  COST: ABS penalty (also penalises s above 0.1); CNT: INEQ constraint (s >= 0.1).  One row of
+   * the Cartesian row buffers per object.  lambda is the damping of the term (the reference's default is 0.1; a
+   * zeroed struct holds 0, so callers set it); it must be finite and >= 0. */
+  double lambda;
 } tb200_term;
 
 /* sco::BasicTrustRegionSQPParameters, optimizers.hpp:92-135 (same defaults via tb200_default_sqp_params) */
@@ -231,7 +238,7 @@ typedef struct tb200_results {
  * Row r of trajectory b linearises one scalar error:  value(q) ~ constant + coeffs.(q - q0)
  * around the waypoint(s) it reads. */
 typedef struct tb200_convexify_out {
-  double* cart_err;         /* [B][n_cart_rows]          coeff-scaled CartPose/CartVel errors at x          */
+  double* cart_err;         /* [B][n_cart_rows]          coeff-scaled CartPose/CartVel/AvoidSingularity errors at x */
   double* cart_jac;         /* [B][n_cart_rows][cart_jac_stride] coeff-scaled Jacobian rows                     */
   double* coll_rows;        /* [B][n_coll_cand][coll_row_stride]: grad[0..nvar-1], dist0, margin, coeff, active */
   double* cost_vals;        /* [B][n_costs]  exact Cost::value(x)           */

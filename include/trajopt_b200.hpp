@@ -228,6 +228,18 @@ struct CartVelTermInfo : TermInfo {
   void hatch(Flat& flat, const ProblemConstructionInfo& pci) const override;
 };
 
+// AvoidSingularityTermInfo, problem_description.hpp:637-659 (without subset_kin_): one object per step on the smallest
+// singular value of `link`'s geometric Jacobian; a TT_COST is an ABS cost, a TT_CNT an INEQ constraint.  hatch throws
+// for more than one coefficient, an unknown link and steps outside the trajectory (the defaults -1 included).
+struct AvoidSingularityTermInfo : TermInfo {
+  std::string link;
+  int first_step = -1, last_step = -1;
+  DblVec coeffs;  // empty: no scaling; one element: the scale of err and gradient
+  double lambda = 0.1;
+  AvoidSingularityTermInfo() { name = "avoid_singularity"; }
+  void hatch(Flat& flat, const ProblemConstructionInfo& pci) const override;
+};
+
 // CollisionTermInfo, problem_description.hpp:600-659 + trajopt_common TrajOptCollisionConfig (collision_types.h:120-170)
 struct CollisionTermInfo : TermInfo {
   int first_step = 0, last_step = -1;
@@ -288,6 +300,20 @@ inline void CartPoseTermInfo::hatch(Flat& flat, const ProblemConstructionInfo& p
   for (int k = 0; k < 4; ++k) t.source_offset[3 + k] = source_frame_offset.wxyz[k];
   t.target_pose[3] = 1.0;  // unused: the target is read from the per-trajectory slot
   t.target_slot = flat.addTargets(target);
+  flat.terms.push_back(t);
+}
+inline void AvoidSingularityTermInfo::hatch(Flat& flat, const ProblemConstructionInfo& pci) const {
+  tb200_term t = detail::blankTerm(TB200_TERM_AVOID_SINGULARITY, term_type, name);
+  const int T = pci.basic_info.n_steps;
+  if (coeffs.size() > 1) throw std::runtime_error(name + ": coeffs has more than one element");
+  if (first_step < 0 || last_step >= T || first_step > last_step)
+    throw std::runtime_error(name + ": steps outside the trajectory");
+  t.first_step = first_step;
+  t.last_step = last_step;
+  t.link = pci.kin->linkIndex(link);
+  t.target_slot = -1;
+  t.coeffs[0] = coeffs.empty() ? 1.0 : coeffs[0];
+  t.lambda = lambda;
   flat.terms.push_back(t);
 }
 inline void CartVelTermInfo::hatch(Flat& flat, const ProblemConstructionInfo& pci) const {

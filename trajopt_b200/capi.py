@@ -15,7 +15,7 @@ MAX_DOF = 16
 JOINT_FIXED, JOINT_REVOLUTE, JOINT_PRISMATIC = 0, 1, 2
 # return codes of the C ABI (include/trajopt_b200.h)
 OK, ERR_INVALID, ERR_UNSUPPORTED, ERR_CUDA, ERR_NO_DEVICE = range(5)
-TERM_JOINT_POS, TERM_JOINT_VEL, TERM_JOINT_ACC, TERM_CART_POSE, TERM_CART_VEL, TERM_COLLISION = range(6)
+TERM_JOINT_POS, TERM_JOINT_VEL, TERM_JOINT_ACC, TERM_CART_POSE, TERM_CART_VEL, TERM_COLLISION, TERM_AVOID_SINGULARITY = range(7)
 ROLE_COST, ROLE_CNT = 1, 2
 COLL_DISCRETE, COLL_LVS_DISCRETE, COLL_CONTINUOUS, COLL_LVS_CONTINUOUS = 1, 2, 3, 4
 OPT_CONVERGED, OPT_SCO_ITERATION_LIMIT, OPT_PENALTY_ITERATION_LIMIT, OPT_TIME_LIMIT, OPT_FAILED, OPT_INVALID = range(6)
@@ -49,7 +49,8 @@ class Term(C.Structure):
                 ("pos_coeffs", C.c_double * 3), ("rot_coeffs", C.c_double * 3), ("max_displacement", C.c_double),
                 ("evaluator_type", C.c_int32), ("n_fixed_steps", C.c_int32), ("fixed_steps", C.c_int32 * 8),
                 ("margin", C.c_double), ("coeff", C.c_double), ("margin_buffer", C.c_double),
-                ("longest_valid_segment_length", C.c_double)]
+                ("longest_valid_segment_length", C.c_double),
+                ("lambda_", C.c_double)]  # AvoidSingularity damping ("lambda" in the C header)
 
 
 class SqpParams(C.Structure):

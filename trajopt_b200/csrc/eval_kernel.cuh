@@ -25,12 +25,16 @@ __host__ __device__ inline int eval_job_stride(int S) { return (S * kFrameStride
 
 struct EvalSmem {
   // offsets in doubles into the dynamic shared buffer
-  int x, sph, spo, jax, velp, objv, mask, misc, fr, terms, obst, sphr, segs, sphs, cobj, aobj, wscr, wscr_stride, cfk, total;
+  int x, sph, spo, jax, velp, objv, mask, misc, fr, terms, obst, sphr, segs, sphs, cobj, aobj, wscr, wscr_stride, cfk, sing, total;
 };
+// per-warp scratch of the AvoidSingularity objects: J(q) column by column ([D][6]), then u[6] and v[D] of its smallest
+// singular value
+__host__ __device__ inline int sing_scratch_stride(int D) { return (7 * D + 6 + 1) & ~1; }
 // n_vel_objs: CartVel step pairs; cast: the collision objects are step pairs (continuous evaluator), each holding at
-// most cast_cap active contacts
+// most cast_cap active contacts; n_sing_objs: AvoidSingularity objects (their scratch is planned only when there are any)
 __host__ __device__ inline EvalSmem eval_smem_layout(int T, int D, int L, int n_coll_objs, int n_mask_words, int S,
-                                                      int n_joint_objs, int n_vel_objs, int cast, int cast_cap, int n_objs) {
+                                                      int n_joint_objs, int n_vel_objs, int cast, int cast_cap, int n_objs,
+                                                      int n_sing_objs = 0) {
   EvalSmem s;
   int o = 0;
   s.x = o;      o += T * D;
@@ -66,6 +70,7 @@ __host__ __device__ inline EvalSmem eval_smem_layout(int T, int D, int L, int n_
   const int st = (((D + 3) & 1) == 0 && !cast) ? 8 * 32 * (D + 3) : 0;  // one staging tile (32 rows) per warp
   o += a > st ? a : st;
   o += o & 1;
+  s.sing = o;   o += n_sing_objs > 0 ? (kEvalThreads / 32) * sing_scratch_stride(D) : 0;
   s.total = o;
   return s;
 }
@@ -92,6 +97,9 @@ struct EvalExtra {
   int* log_len;                // [B] records written
   int* log_dropped;            // [B] records that did not fit
   int log_cap, log_stride, log_with_x, pad;
+  // AvoidSingularity objects (one per step; coeff: the term's coefficient, margin: its lambda)
+  const DevObj* sing_objs;
+  int n_sing_objs, pad_sing;
 };
 
 #ifdef TB200_EVAL_PROFILE
@@ -202,7 +210,171 @@ static __device__ __noinline__ void log_record_arrays(const DevProblem& p, const
     for (int i = tid; i < p.N; i += kEvalThreads) rec[i] = qp_failed ? qnan : xs[i];
 }
 
+// ---- AvoidSingularity rows (kinematic_terms.cpp:586-642) ------------------------------------------------------------
+// err = 1/(s + lambda) - 1/(0.1 + lambda) with s the smallest singular value of the 6 x D geometric Jacobian J(q) of the
+// link's origin (linear rows, then angular; a zero column for a joint that does not move the link), and the gradient
+// g_j = u' ((J(q + eps e_j) - J(q)) / eps) v * (-1 / (s + lambda)^2), eps = 1e-6, with u, v the singular vectors of s.
+// Both go out scaled by the term's coefficient: one row of the Cartesian buffers per object.
+constexpr double kSingEps = 1e-6;      // AvoidSingularityJacCalculator's eps_
+// Jacobi rotations stop when every |a_p . a_q| <= M eps |a_p| |a_q| (M: the length of the columns; LAPACK's dgesvj
+// uses the same scale): below that the off-diagonal is the rounding of the dot product itself
+constexpr double kSingSvdEps = 2.220446049250313e-16;
+constexpr int kSingSvdSweeps = 32;
+
+// the chain of a link at q + eps e_pj (pj < 0: at q), running frame in registers with the products of the CartPose
+// walk; on_joint(segment, R, p) sees the world frame of every joint segment on the chain.  Returns the link origin.
+template <class OnJoint>
+__device__ __forceinline__ void sing_walk(const DevSegment* segs, const int* chain, const double* qw, const int pj,
+                                          double* pe, OnJoint&& on_joint) {
+  double R[9], P[3];
+  const int clen = chain[0];
+  for (int k = 0; k < clen; ++k) {
+    const DevSegment& g = segs[chain[1 + k]];
+    const double qv = (g.q_index >= 0) ? qw[g.q_index] + (g.q_index == pj ? kSingEps : 0.0) : 0.0;
+    Frame loc;
+    segment_local_q(g, qv, loc);
+    if (k == 0) {
+#pragma unroll
+      for (int i = 0; i < 9; ++i) R[i] = loc.R[i];
+#pragma unroll
+      for (int i = 0; i < 3; ++i) P[i] = loc.p[i];
+    } else {
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        const double r0 = R[i * 3], r1 = R[i * 3 + 1], r2 = R[i * 3 + 2], rp = P[i];
+        R[i * 3 + 0] = r0 * loc.R[0] + r1 * loc.R[3] + r2 * loc.R[6];
+        R[i * 3 + 1] = r0 * loc.R[1] + r1 * loc.R[4] + r2 * loc.R[7];
+        R[i * 3 + 2] = r0 * loc.R[2] + r1 * loc.R[5] + r2 * loc.R[8];
+        P[i] = r0 * loc.p[0] + r1 * loc.p[1] + r2 * loc.p[2] + rp;
+      }
+    }
+    if (g.q_index >= 0) on_joint(g, R, P);
+  }
+#pragma unroll
+  for (int i = 0; i < 3; ++i) pe[i] = P[i];
+}
+
+// column of the geometric Jacobian at the link origin pe for a joint with world frame (R, P): [a x (pe - o); a]
+// (revolute) or [a; 0] (prismatic), a = R * axis, o = P
+__device__ __forceinline__ void sing_column(const DevSegment& g, const double* R, const double* P, const double* pe,
+                                            double* col) {
+  double a[3];
+#pragma unroll
+  for (int i = 0; i < 3; ++i) a[i] = R[i * 3] * g.axis[0] + R[i * 3 + 1] * g.axis[1] + R[i * 3 + 2] * g.axis[2];
+  if (g.joint_type == 1) {
+    const double d0 = pe[0] - P[0], d1 = pe[1] - P[1], d2 = pe[2] - P[2];
+    col[0] = a[1] * d2 - a[2] * d1; col[1] = a[2] * d0 - a[0] * d2; col[2] = a[0] * d1 - a[1] * d0;
+    col[3] = a[0]; col[4] = a[1]; col[5] = a[2];
+  } else {
+    col[0] = a[0]; col[1] = a[1]; col[2] = a[2];
+    col[3] = 0.0; col[4] = 0.0; col[5] = 0.0;
+  }
+}
+
+// sum over the warp, the same bits in every lane (lane 0's butterfly result, broadcast)
+__device__ __forceinline__ double sing_warp_sum(double v) {
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+  return __shfl_sync(0xffffffffu, v, 0);
+}
+
+// One warp per object (objects warp, warp + 8, ...).  Lane 0 builds J(q) in shared memory; the warp runs a one-sided
+// Jacobi SVD on it (on J's D columns when D < 6, else on the 6 columns of J', one row of the rotated matrix per lane,
+// rotations in a fixed cyclic order); lane 1 + j then walks the chain at q + eps e_j and projects its difference
+// columns on u, v as it meets them.  Called only by the SING instances of the evaluation step.
 template <int DD>
+static __device__ __noinline__ void singularity_objects(const EvalExtra& ex, const double* xs, const DevSegment* segs,
+                                                        double* scratch, double* err_out, double* jac_out, const int stride) {
+  constexpr int D = DD;
+  constexpr int NC = D < 6 ? D : 6;  // columns the rotations act on
+  constexpr int M = D < 6 ? 6 : D;   // their length
+  constexpr double tol = M * kSingSvdEps;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double* J0 = scratch + warp * sing_scratch_stride(D);
+  double* uu = J0 + 6 * D;
+  double* vv = uu + 6;
+  for (int c = warp; c < ex.n_sing_objs; c += kEvalThreads / 32) {
+    const DevObj& o = ex.sing_objs[c];
+    const int* chain = ex.link_chain + o.link * (kMaxSeg + 1);
+    const double* qw = xs + o.first * D;
+    const int pj = lane - 1;  // lane 0: J(q); lane 1 + j: J(q + eps e_j)
+    const bool work = lane <= D;
+    double pe[3] = {0.0, 0.0, 0.0};
+    if (work) sing_walk(segs, chain, qw, pj, pe, [](const DevSegment&, const double*, const double*) {});
+    for (int i = lane; i < 6 * D; i += 32) J0[i] = 0.0;
+    __syncwarp();
+    if (lane == 0)
+      sing_walk(segs, chain, qw, -1, pe, [&](const DevSegment& g, const double* R, const double* P) {
+        sing_column(g, R, P, pe, J0 + 6 * g.q_index);
+      });
+    __syncwarp();
+    // ---- one-sided Jacobi: A V = W with orthogonal columns; A = J (D < 6) or J' (D >= 6), lane i holds row i ----
+    double a[NC], vr[NC];
+#pragma unroll
+    for (int k = 0; k < NC; ++k) {
+      a[k] = lane < M ? (D < 6 ? J0[k * 6 + lane] : J0[lane * 6 + k]) : 0.0;
+      vr[k] = (lane == k) ? 1.0 : 0.0;
+    }
+    for (int sweep = 0; sweep < kSingSvdSweeps; ++sweep) {
+      bool rotated = false;
+#pragma unroll
+      for (int pa = 0; pa < NC - 1; ++pa) {
+#pragma unroll
+        for (int qa = pa + 1; qa < NC; ++qa) {
+          const double al = sing_warp_sum(a[pa] * a[pa]), be = sing_warp_sum(a[qa] * a[qa]), ga = sing_warp_sum(a[pa] * a[qa]);
+          if (fabs(ga) > tol * sqrt(al * be)) {  // (warp-uniform)
+            const double zeta = (be - al) / (2.0 * ga);
+            const double t = (zeta >= 0.0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
+            const double cs = 1.0 / sqrt(1.0 + t * t), sn = cs * t;
+            const double ap = a[pa], aq = a[qa], vp = vr[pa], vq = vr[qa];
+            a[pa] = cs * ap - sn * aq; a[qa] = sn * ap + cs * aq;
+            vr[pa] = cs * vp - sn * vq; vr[qa] = sn * vp + cs * vq;
+            rotated = true;
+          }
+        }
+      }
+      if (!rotated) break;
+    }
+    // the smallest singular value: the shortest column of W
+    double sigma = 0.0, ak = 0.0, vk = 0.0;
+#pragma unroll
+    for (int k = 0; k < NC; ++k) {
+      const double sk = sqrt(sing_warp_sum(a[k] * a[k]));
+      if (k == 0 || sk < sigma) { sigma = sk; ak = a[k]; vk = vr[k]; }
+    }
+    // s = 0 leaves the direction W_k / s undefined: that vector is taken as 0 (the gradient is then 0)
+    const double wk = sigma > 0.0 ? ak / sigma : 0.0;
+    if (D < 6) {  // u = W_k / s, v = V_k
+      if (lane < 6) uu[lane] = wk;
+      if (lane < D) vv[lane] = vk;
+    } else {      // J' = W V': u = V_k, v = W_k / s
+      if (lane < 6) uu[lane] = vk;
+      if (lane < D) vv[lane] = wk;
+    }
+    __syncwarp();
+    const double coeff = o.coeff, lam = o.margin;
+    if (lane == 0) err_out[o.src_off] = coeff * (1.0 / (sigma + lam) - 1.0 / (0.1 + lam));
+    if (work && lane > 0) {
+      double g = 0.0, pk[3];  // (pe: this lane's link origin from the first walk)
+      sing_walk(segs, chain, qw, pj, pk, [&](const DevSegment& sg, const double* R, const double* P) {
+        double col[6];
+        sing_column(sg, R, P, pe, col);
+        const double* c0 = J0 + 6 * sg.q_index;
+        double s = 0.0;
+#pragma unroll
+        for (int i = 0; i < 6; ++i) s += uu[i] * ((col[i] - c0[i]) / kSingEps);
+        g += s * vv[sg.q_index];
+      });
+      g *= -1.0 / ((sigma + lam) * (sigma + lam));
+      jac_out[static_cast<size_t>(o.src_off) * stride + pj] = coeff * g;
+    }
+    __syncwarp();  // the scratch of the warp is reused by its next object
+  }
+}
+
+// SING: the instance for problems with AvoidSingularity objects (every other problem runs SING = 0, whose code has
+// none of the term's)
+template <int DD, int SING>
 __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalExtra& ex, const int mode, const int b,
                                                const double* x_in /*EVAL_ONLY*/, bool& tables_ready) {
   extern __shared__ double sm[];
@@ -216,7 +388,7 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
   if (tid == 0 && !qp_failed) atomicAdd(p.active_count + 1, 1);  // trajectories actually convexified (bench: bytes moved)
   const int n_mask_words = p.n_coll_objs * p.coll_words;
   const EvalSmem S = eval_smem_layout(T, D, L, p.n_coll_objs, n_mask_words, p.S, ex.n_joint_objs, ex.n_vel_objs,
-                                      ex.cast, ex.cast_cap, p.n_costs + p.n_cnts);
+                                      ex.cast, ex.cast_cap, p.n_costs + p.n_cnts, SING ? ex.n_sing_objs : 0);
   static_assert(sizeof(DevObj) % 8 == 0 && sizeof(DevSegment) % 8 == 0 && sizeof(DevSphere) % 8 == 0, "tables are copied as doubles");
   const DevObj* cobjs = reinterpret_cast<const DevObj*>(sm + S.cobj);
   const DevObj* aobjs = reinterpret_cast<const DevObj*>(sm + S.aobj);
@@ -857,6 +1029,10 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
       }
       if (lane_c == 0) sm[S.objv + k] = vsum;
     }
+    // ---- AvoidSingularity rows: a warp per object, as its collision work runs out ----
+    if constexpr (SING != 0)
+      singularity_objects<D>(ex, xs, segs, sm + S.sing, p.cart_err + slot * p.n_cart_rows,
+                             p.cart_jac + slot * p.n_cart_rows * p.cart_stride, p.cart_stride);
     __syncthreads();
     EVAL_PROF(5);
     for (int i = tid; i < n_mask_words; i += kEvalThreads) p.coll_mask[slot * n_mask_words + i] = mask[i];
@@ -889,6 +1065,9 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
       } else if (o.kind == OBJ_CART_VEL) {
         const double* e = p.cart_err + slot * p.n_cart_rows + o.src_off;
         for (int r = 0; r < 6; ++r) v += is_cnt ? fmax(e[r], 0.0) : fabs(e[r]);  // INEQ violation | ABS cost
+      } else if (SING != 0 && o.kind == OBJ_SINGULARITY) {
+        const double e = p.cart_err[slot * p.n_cart_rows + o.src_off];
+        v = is_cnt ? fmax(e, 0.0) : fabs(e);  // INEQ violation | ABS cost
       } else {
         v = sm[S.objv + o.kernel_slot];  // collision object: summed by the warp that built its rows
       }
@@ -1076,11 +1255,11 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
 
 // The evaluation step as a function of its own (the persistent SQP kernel calls it beside its QP step; the stand-alone
 // kernel below inlines the implementation).
-template <int DD>
+template <int DD, int SING = 0>
 __device__ __noinline__ void eval_step(const DevProblem& p, const EvalExtra& ex, const int mode, const int b,
                                        const double* x_in /*EVAL_ONLY*/) {
   bool tables_ready = false;  // (the QP step used the same shared memory in between)
-  eval_step_impl<DD>(p, ex, mode, b, x_in, tables_ready);
+  eval_step_impl<DD, SING>(p, ex, mode, b, x_in, tables_ready);
 }
 
 // Two CTAs per SM cap the 7-joint instance at 128 registers, and on sm_90a ptxas spills a few of them; one CTA per SM
@@ -1091,7 +1270,7 @@ __device__ __noinline__ void eval_step(const DevProblem& p, const EvalExtra& ex,
 #endif
 // Stand-alone launch, one CTA per trajectory: the initial evaluation of a solve (EVAL_INIT) and the kernel-level
 // convexify entry point (EVAL_ONLY).  Inside a solve the same code runs as a step of solve_kernel.cuh.
-template <int DD>
+template <int DD, int SING = 0>
 __global__ void __launch_bounds__(kEvalThreads, (DD <= 8) ? TB200_EVAL_MIN_BLOCKS : 2)
 eval_convexify_decide_kernel(const __grid_constant__ DevProblem p, const __grid_constant__ EvalExtra ex, int mode,
                              const double* x_in /*EVAL_ONLY*/) {
@@ -1105,7 +1284,7 @@ eval_convexify_decide_kernel(const __grid_constant__ DevProblem p, const __grid_
     const int b = s_next;
     __syncthreads();
     if (b >= p.B) return;
-    eval_step_impl<DD>(p, ex, mode, b, x_in, tables_ready);
+    eval_step_impl<DD, SING>(p, ex, mode, b, x_in, tables_ready);
     __syncthreads();
   }
 }

@@ -5,13 +5,13 @@
 #include "kernels.h"
 
 namespace tb200 {
-EvalKernelFn eval_kernel_for(int D) {
+EvalKernelFn eval_kernel_for(int D, bool sing) {
   switch (D) {
-    case 2: return eval_convexify_decide_kernel<2>;
-    case 3: return eval_convexify_decide_kernel<3>;
-    case 6: return eval_convexify_decide_kernel<6>;
-    case 7: return eval_convexify_decide_kernel<7>;
-    case 14: return eval_convexify_decide_kernel<14>;
+    case 2: return sing ? eval_convexify_decide_kernel<2, 1> : eval_convexify_decide_kernel<2>;
+    case 3: return sing ? eval_convexify_decide_kernel<3, 1> : eval_convexify_decide_kernel<3>;
+    case 6: return sing ? eval_convexify_decide_kernel<6, 1> : eval_convexify_decide_kernel<6>;
+    case 7: return sing ? eval_convexify_decide_kernel<7, 1> : eval_convexify_decide_kernel<7>;
+    case 14: return sing ? eval_convexify_decide_kernel<14, 1> : eval_convexify_decide_kernel<14>;
     default: return nullptr;
   }
 }

@@ -32,6 +32,7 @@ struct FlatProblem {
   // copies of the CartPose, CartVel and collision objects for the evaluation kernel; collision objects in the order the
   // QP kernel meets them (costs first), which is also the order of their candidates
   std::vector<DevObj> cart_objs, vel_objs, coll_objs;
+  std::vector<DevObj> sing_objs;  // avoid_singularity objects (one per step) for the evaluation kernel
   std::vector<DevJointTerm> joint_terms;
   std::vector<DevCartTerm> cart_terms;
   std::vector<int> fixed_vars;
@@ -125,8 +126,9 @@ inline int fold_robot(const tb200_problem_desc& d, FlatProblem& F, std::vector<i
     used[g] = 1;
   }
   for (int k = 0; k < d.n_terms; ++k)
-    if ((d.terms[k].kind == TB200_TERM_CART_POSE || d.terms[k].kind == TB200_TERM_CART_VEL) && d.terms[k].link >= 0 &&
-        d.terms[k].link < S)
+    if ((d.terms[k].kind == TB200_TERM_CART_POSE || d.terms[k].kind == TB200_TERM_CART_VEL ||
+         d.terms[k].kind == TB200_TERM_AVOID_SINGULARITY) &&
+        d.terms[k].link >= 0 && d.terms[k].link < S)
       used[d.terms[k].link] = 1;
   remap.assign(S, -1);
   std::vector<DevSegment> acc(S);  // transform from the nearest kept ancestor's frame to this (folded) segment
@@ -179,7 +181,7 @@ struct Lists {
   using Ref = std::pair<Id, int>;
   std::vector<DevObj> obj[3];
   std::vector<std::pair<int, int>> src[3];
-  std::vector<Ref> cart, vel, coll;
+  std::vector<Ref> cart, vel, coll, sing;
   Ref add(Id l, const DevObj& o, int term, int step) {
     obj[l].push_back(o);
     src[l].push_back({term, step});
@@ -295,6 +297,28 @@ inline int hatch_terms(const tb200_problem_desc& d, const std::vector<int>& rema
         F.has_vel = true;
         lists.vel.push_back(lists.add(is_cnt ? Lists::INEQ : Lists::COST, c, k, t));
       }
+    } else if (tm.kind == TB200_TERM_AVOID_SINGULARITY) {
+      // AvoidSingularityTermInfo::hatch (problem_description.cpp:1900-1939): one object per step over its D joints, an
+      // ABS cost or an INEQ constraint; fixed timesteps are not skipped.  (The reference's defaults first_step =
+      // last_step = -1 would index step -1: refused here.)
+      if (tm.link < 0 || tm.link >= d.robot.n_segments) return refuse(msg, TB200_ERR_INVALID, "avoid_singularity link out of range");
+      if (tm.first_step < 0 || tm.last_step >= T || tm.first_step > tm.last_step)
+        return refuse(msg, TB200_ERR_INVALID, "avoid_singularity steps outside the trajectory");
+      if (!std::isfinite(tm.lambda) || tm.lambda < 0.0)
+        return refuse(msg, TB200_ERR_INVALID, "avoid_singularity lambda must be finite and >= 0");
+      for (int t = tm.first_step; t <= tm.last_step; ++t) {
+        DevObj c = o;
+        c.kind = OBJ_SINGULARITY;
+        c.first = t;
+        c.link = remap[tm.link];
+        c.src_off = F.n_cart_rows;
+        c.n_rows = 1;
+        c.coeff = tm.coeffs[0];
+        c.margin = tm.lambda;
+        F.n_cart_rows += 1;
+        F.max_rows += 1;
+        lists.sing.push_back(lists.add(is_cnt ? Lists::INEQ : Lists::COST, c, k, t));
+      }
     } else {
       return refuse(msg, TB200_ERR_INVALID, "unknown term kind");
     }
@@ -319,6 +343,7 @@ inline void order_objects(Lists& lists, FlatProblem& F) {
   };
   for (Lists::Ref r : lists.cart) F.cart_objs.push_back(copy(r));
   for (Lists::Ref r : lists.vel) F.vel_objs.push_back(copy(r));
+  for (Lists::Ref r : lists.sing) F.sing_objs.push_back(copy(r));
   for (const bool costs : {true, false})
     for (Lists::Ref r : lists.coll) {
       if (costs != (r.first == Lists::COST)) continue;

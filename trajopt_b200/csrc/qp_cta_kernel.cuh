@@ -3110,7 +3110,42 @@ __device__ inline QpOut qp_solve_block(QpCtx& q, const QpSettings& st, bool warm
 // ---------------------------------------------------------------------------------------------------
 // QP assembly (optimizers.cpp:781-799 + osqp_interface.cpp:170-281 in fixed layout) + solve of trajectory b by the
 // calling CTA (256 threads).  DD = degrees of freedom (block size NB = 2*DD); PAIR: rows may span two waypoints.
-template <int DD, int PAIR>
+// The row of an AvoidSingularity object (problem_description.cpp:1900-1939): 1 row over q_first, D coefficients; an ABS
+// cost row or an INEQ constraint row (hinge), the coefficients with |g| <= 1e-7 of the unscaled gradient dropped
+// (cleanupAff, modeling_utils.cpp:143-211, 238-269).  Written by thread 0; returns the row's entries of A (its real
+// coefficients and aux columns).  Called only by the SING instances of qp_step.
+static __device__ __noinline__ int qp_singularity_row(const DevProblem& p, const QpCtx& q, const DevObj& o, const int oi,
+                                                      const bool is_cnt, const double w_aux, const double* cart_err,
+                                                      const double* cart_jac, const int nr, const int n_aux, int* sh_i) {
+  const int D = q.D;
+  if (q.tid == 0) {
+    double* R = q.R(nr);
+    int* I = q.rints + static_cast<size_t>(nr) * RI_NINTS;
+    const double* J = cart_jac + static_cast<size_t>(o.src_off) * p.cart_stride;
+    const double thr = 1e-7 * fabs(o.coeff);
+    double dot = 0.0;
+    int nz = 0;
+    for (int j = 0; j < q.CN; ++j) {
+      const double Jj = (j < D) ? J[j] : 0.0;
+      dot += Jj * q.x[o.first * D + min(j, D - 1)];
+      const double a = (fabs(Jj) > thr) ? Jj : 0.0;
+      R[j] = a;
+      nz += (a != 0.0);
+    }
+    R[2 * q.CN + R_C] = cart_err[o.src_off] - dot;
+    R[2 * q.CN + R_W] = w_aux;
+    I[RI_BASE] = o.first * D; I[RI_CNT] = D; I[RI_STRIDE] = 1; I[RI_AUX] = is_cnt ? AUX_HINGE : AUX_ABS;
+    I[RI_OBJ] = oi; I[RI_PAD] = n_aux;
+    sh_i[0] = nz;
+  }
+  __syncthreads();
+  const int nz = sh_i[0];
+  __syncthreads();
+  return nz + (is_cnt ? 1 : 2);
+}
+
+// SING: the instance for problems with AvoidSingularity objects (the row builder of SING = 0 has no branch for them)
+template <int DD, int PAIR, int SING = 0>
 __device__ __noinline__ void qp_step(const DevProblem& p, const int b, const double* x_override /*kernel-level API*/,
                                         const double* trust_override, int* admm_iters_out, int* polish_out) {
   constexpr int NB = 2 * DD;
@@ -3302,6 +3337,10 @@ __device__ __noinline__ void qp_step(const DevProblem& p, const int b, const dou
         nr += 6;
         n_aux += per * 6;
         nnzA += nz + per * 6;
+      } else if (SING != 0 && o.kind == OBJ_SINGULARITY) {
+        nnzA += qp_singularity_row(p, q, o, oi, is_cnt, w_aux, cart_err, cart_jac, nr, n_aux, sh_i);
+        nr += 1;
+        n_aux += is_cnt ? 1 : 2;
       } else if (o.kind == OBJ_COLL || o.kind == OBJ_COLL_CAST) {
         // active candidates of this timestep, in candidate order: thread 0 scans the mask and assigns slots
         const unsigned long long* mw = coll_mask + static_cast<size_t>(coll_obj_counter) * p.coll_words;

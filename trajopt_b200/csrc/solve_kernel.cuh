@@ -123,7 +123,8 @@ __device__ inline bool stopped_at_iteration_top(const DevProblem& p, const int b
 }
 constexpr double kNoTimeLimit = 1.7976931348623157e308;  // DBL_MAX, tb200_default_sqp_params
 
-template <int DD, int PAIR>
+// SING: the instance for problems with AvoidSingularity objects (solve_inst_<D>_<PAIR>_sing.cu)
+template <int DD, int PAIR, int SING = 0>
 __global__ void __launch_bounds__(kQpThreads, 1)
 solve_kernel(const __grid_constant__ DevProblem p, const __grid_constant__ EvalExtra ex, const __grid_constant__ SolveCtl ctl) {
   const int tid = threadIdx.x;
@@ -143,11 +144,11 @@ solve_kernel(const __grid_constant__ DevProblem p, const __grid_constant__ EvalE
       }
       const unsigned long long t0 = global_ns();
       // (a single call site: the QP solve stays inlined in the kernel, as tuned)
-      qp_step<DD, PAIR>(p, b, ctl.x_override, ctl.trust_override, ctl.admm_iters_out, ctl.polish_out);
+      qp_step<DD, PAIR, SING>(p, b, ctl.x_override, ctl.trust_override, ctl.admm_iters_out, ctl.polish_out);
       if (qp_only) break;
       __syncthreads();
       const unsigned long long t1 = global_ns();
-      eval_step<DD>(p, ex, EVAL_STEP, b, nullptr);
+      eval_step<DD, SING>(p, ex, EVAL_STEP, b, nullptr);
       __syncthreads();
       const unsigned long long t2 = global_ns();
       t_qp += t1 - t0;

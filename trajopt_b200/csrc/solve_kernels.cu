@@ -7,13 +7,14 @@ namespace tb200 {
 #define TB200_INSTANCES(X) X(2, 0) X(3, 0) X(6, 0) X(7, 0) X(14, 0) X(2, 1) X(7, 1)
 #define TB200_DECL(D, P)                  \
   SolveKernelFn solve_kernel_inst_##D##_##P(); \
+  SolveKernelFn solve_kernel_sing_inst_##D##_##P(); \
   int qp_prof_inst_##D##_##P(unsigned long long*, int);
 TB200_INSTANCES(TB200_DECL)
 #undef TB200_DECL
 
-SolveKernelFn solve_kernel_for(int D, bool pair_rows) {
+SolveKernelFn solve_kernel_for(int D, bool pair_rows, bool sing) {
 #define TB200_PICK(DD, P) \
-  if (D == DD && pair_rows == static_cast<bool>(P)) return solve_kernel_inst_##DD##_##P();
+  if (D == DD && pair_rows == static_cast<bool>(P)) return sing ? solve_kernel_sing_inst_##DD##_##P() : solve_kernel_inst_##DD##_##P();
   TB200_INSTANCES(TB200_PICK)
 #undef TB200_PICK
   return nullptr;

@@ -67,11 +67,12 @@ struct tb200_problem {
   DevBuf<double> log;
   DevBuf<int> log_len, log_dropped;
   bool pair_rows = false;  // QP rows span two waypoints (CartVel, continuous collision): 2*D coefficients per row
+  bool sing = false;       // AvoidSingularity objects: the kernel instances with the term (SING = 1)
   // device storage
   DevBuf<DevSegment> segs;
   DevBuf<DevSphere> spheres;
   DevBuf<double> lower, upper, Pband, qlin, init_traj, cart_targets, obstacles;
-  DevBuf<DevObj> d_cost_objs, d_cnt_objs, d_cart_objs, d_coll_objs, d_vel_objs;
+  DevBuf<DevObj> d_cost_objs, d_cnt_objs, d_cart_objs, d_coll_objs, d_vel_objs, d_sing_objs;
   DevBuf<DevJointTerm> joint_terms;
   DevBuf<DevCartTerm> cart_terms;
   DevBuf<int> fixed_vars;
@@ -157,6 +158,8 @@ int planLayout(const tb200_problem_desc& d, const FlatProblem& F, tb200_problem&
   ex.n_cart_objs = static_cast<int>(F.cart_objs.size());
   ex.n_coll_objs = dp.n_coll_objs;
   ex.n_vel_objs = static_cast<int>(F.vel_objs.size());
+  ex.n_sing_objs = static_cast<int>(F.sing_objs.size());
+  P.sing = ex.n_sing_objs > 0;
   ex.cast = F.has_cast ? 1 : 0;
   ex.cast_cap = F.cast_cap;
   ex.n_joint_objs = F.n_joint_objs;
@@ -166,7 +169,7 @@ int planLayout(const tb200_problem_desc& d, const FlatProblem& F, tb200_problem&
   std::copy(std::begin(F.sphere_jmask), std::end(F.sphere_jmask), ex.sphere_jmask);
 
   const EvalSmem es = eval_smem_layout(T, D, dp.L, dp.n_coll_objs, dp.n_coll_objs * dp.coll_words, dp.S, ex.n_joint_objs,
-                                       ex.n_vel_objs, ex.cast, ex.cast_cap, dp.n_costs + dp.n_cnts);
+                                       ex.n_vel_objs, ex.cast, ex.cast_cap, dp.n_costs + dp.n_cnts, ex.n_sing_objs);
   P.pair_rows = (CN > std::max(D, 3));
   P.eval_smem = static_cast<size_t>(es.total) * sizeof(double);
   const bool factor_global = D > 8;  // = FG of qp_step: blocks of 2*D > 16 never fit
@@ -178,7 +181,7 @@ int planLayout(const tb200_problem_desc& d, const FlatProblem& F, tb200_problem&
   if (P.eval_smem > 226 * 1024 || P.qp_smem > 226 * 1024)
     return fail(TB200_ERR_UNSUPPORTED, "problem does not fit the 227 KB shared memory of one CTA");
   if (CN > 32) return fail(TB200_ERR_UNSUPPORTED, "more than 32 coefficients per QP row");
-  if (!solve_kernel_for(D, P.pair_rows) || !eval_kernel_for(D))
+  if (!solve_kernel_for(D, P.pair_rows, P.sing) || !eval_kernel_for(D, P.sing))
     return fail(TB200_ERR_UNSUPPORTED, P.pair_rows ? "no kernel instance with two-waypoint rows (CartVel, continuous collision) for this number of joints"
                                                    : "no kernel instance for this number of joints");
   return TB200_OK;
@@ -198,14 +201,14 @@ int setupDevice(tb200_problem& P, int device) {
     CK(cudaDeviceGetLimit(&cur, cudaLimitStackSize));
     if (cur < 6144) CK(cudaDeviceSetLimit(cudaLimitStackSize, 6144));
   }
-  CK(cudaFuncSetAttribute(eval_kernel_for(P.D), cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(P.eval_smem)));
+  CK(cudaFuncSetAttribute(eval_kernel_for(P.D, P.sing), cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(P.eval_smem)));
   P.solve_smem = std::max(P.qp_smem, P.eval_smem);  // the QP step and the evaluation step share one buffer
-  CK(cudaFuncSetAttribute(solve_kernel_for(P.D, P.pair_rows), cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(P.solve_smem)));
+  CK(cudaFuncSetAttribute(solve_kernel_for(P.D, P.pair_rows, P.sing), cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(P.solve_smem)));
   int sms = 0;
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
   P.n_sm = std::max(1, sms);
   int per_sm = 1;
-  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, eval_kernel_for(P.D), kEvalThreads, P.eval_smem));
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, eval_kernel_for(P.D, P.sing), kEvalThreads, P.eval_smem));
   P.eval_grid = std::max(1, std::min(P.B, std::max(1, per_sm) * P.n_sm));
   if (const char* e = std::getenv("TB200_QUANTUM")) P.quantum = std::max(1, std::atoi(e));
   // TB200_GENERIC_QP_PASSES=1: termination checks and polish refinement by the generic passes of the QP solver instead
@@ -244,6 +247,7 @@ int allocate(const tb200_problem_desc& d, FlatProblem& F, tb200_problem& P) {
   ex.cart_objs = upload(P.d_cart_objs, F.cart_objs);
   ex.coll_objs = upload(P.d_coll_objs, F.coll_objs);
   ex.vel_objs = upload(P.d_vel_objs, F.vel_objs);
+  ex.sing_objs = upload(P.d_sing_objs, F.sing_objs);
   dp.joint_terms = upload(P.joint_terms, F.joint_terms);
   dp.cart_terms = upload(P.cart_terms, F.cart_terms);
   dp.fixed_vars = upload(P.fixed_vars, F.fixed_vars);
@@ -579,7 +583,7 @@ int tb200_solve_batch_resident(tb200_problem* P) {
   // the initial evaluation + convexification of every trajectory: one CTA per trajectory (optimizers.cpp:761-783)
   CK(cudaEventRecord(e_init0, st));
   CK(cudaMemsetAsync(P->work_counter.p, 0, sizeof(int), st));
-  eval_kernel_for(P->D)<<<P->eval_grid, kEvalThreads, P->eval_smem, st>>>(dp, P->ex, EVAL_INIT, nullptr);
+  eval_kernel_for(P->D, P->sing)<<<P->eval_grid, kEvalThreads, P->eval_smem, st>>>(dp, P->ex, EVAL_INIT, nullptr);
   CK(cudaEventRecord(e_init1, st));
   // everything else: one persistent CTA per SM (solve_kernel.cuh); no host round trips until every trajectory is done
   SolveCtl ctl{};
@@ -587,7 +591,7 @@ int tb200_solve_batch_resident(tb200_problem* P) {
   ctl.quantum = P->quantum;
   ctl.sched_state = dp.sched_state;
   ctl.timers = dp.sched_timers;
-  solve_kernel_for(P->D, P->pair_rows)<<<std::min(dp.B, P->n_sm), kQpThreads, P->solve_smem, st>>>(dp, P->ex, ctl);
+  solve_kernel_for(P->D, P->pair_rows, P->sing)<<<std::min(dp.B, P->n_sm), kQpThreads, P->solve_smem, st>>>(dp, P->ex, ctl);
   // the best seed of every group, inside the timed region (without groups the identity selection is made only when
   // tb200_fetch_group_results asks for it)
   P->solved_group_size = dp.group_size;
@@ -701,7 +705,7 @@ int tb200_convexify_batch(tb200_problem* P, const double* x, tb200_convexify_out
   CK(cudaMemsetAsync(P->work_counter.p, 0, sizeof(int), st));
   cudaEvent_t e0 = getEvent(P, 0), e1 = getEvent(P, 1);
   CK(cudaEventRecord(e0, st));
-  eval_kernel_for(P->D)<<<P->eval_grid, kEvalThreads, P->eval_smem, st>>>(dp, P->ex, EVAL_ONLY, P->x_tmp.p);
+  eval_kernel_for(P->D, P->sing)<<<P->eval_grid, kEvalThreads, P->eval_smem, st>>>(dp, P->ex, EVAL_ONLY, P->x_tmp.p);
   CK(cudaEventRecord(e1, st));
   CK(cudaGetLastError());
   {  // device time and algorithmic bytes of this one full-batch launch (bench.py: roofline of the kernel)
@@ -736,13 +740,13 @@ int tb200_qp_solve_batch(tb200_problem* P, const double* x, const double* trust,
   CK(cudaMemsetAsync(P->lvs_overflow.p, 0, B * sizeof(int), st));
   CK(cudaMemsetAsync(P->work_counter.p, 0, sizeof(int), st));
   if (dp.qp_paths) CK(cudaMemsetAsync(dp.qp_paths, 0, B * sizeof(int), st));
-  eval_kernel_for(P->D)<<<P->eval_grid, kEvalThreads, P->eval_smem, st>>>(dp, P->ex, EVAL_ONLY, P->x_tmp.p);
+  eval_kernel_for(P->D, P->sing)<<<P->eval_grid, kEvalThreads, P->eval_smem, st>>>(dp, P->ex, EVAL_ONLY, P->x_tmp.p);
   SolveCtl ctl{};
   ctl.mode = SOLVE_QP_ONLY;  // one QP step per trajectory (one CTA each), no evaluation / decision
   ctl.quantum = 1;
   ctl.x_override = P->x_tmp.p; ctl.trust_override = P->trust_tmp.p;
   ctl.admm_iters_out = P->tmp_iters.p; ctl.polish_out = P->tmp_polish.p;
-  solve_kernel_for(P->D, P->pair_rows)<<<std::min(dp.B, P->n_sm), kQpThreads, P->solve_smem, st>>>(dp, P->ex, ctl);
+  solve_kernel_for(P->D, P->pair_rows, P->sing)<<<std::min(dp.B, P->n_sm), kQpThreads, P->solve_smem, st>>>(dp, P->ex, ctl);
   CK(cudaGetLastError());
   CK(pull(P, new_x, dp.new_x, B * dp.N * sizeof(double)));
   CK(pull(P, qp_status, dp.qp_status, B * sizeof(int)));

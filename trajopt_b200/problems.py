@@ -6,8 +6,8 @@ inputs fed to both the CUDA path and the CPU oracle.
 import numpy as np
 
 from . import capi, robots
-from .capi import (COLL_DISCRETE, COLL_LVS_CONTINUOUS, ROLE_CNT, ROLE_COST, TERM_CART_POSE, TERM_CART_VEL, TERM_COLLISION,
-                   TERM_JOINT_ACC, TERM_JOINT_POS, TERM_JOINT_VEL, ProblemDesc, Term)
+from .capi import (COLL_DISCRETE, COLL_LVS_CONTINUOUS, ROLE_CNT, ROLE_COST, TERM_AVOID_SINGULARITY, TERM_CART_POSE,
+                   TERM_CART_VEL, TERM_COLLISION, TERM_JOINT_ACC, TERM_JOINT_POS, TERM_JOINT_VEL, ProblemDesc, Term)
 
 SEED = 20260923
 
@@ -49,6 +49,17 @@ def cart_pose_term(role, timestep, link, target_slot=-1, target_pose=None, pos_c
     t.target_pose[:] = target_pose if target_pose is not None else (0, 0, 0, 1, 0, 0, 0)
     t.pos_coeffs[:] = pos_coeffs
     t.rot_coeffs[:] = rot_coeffs
+    return t
+
+
+def avoid_singularity_term(role, first, last, link, coeff=1.0, lam=0.1):
+    """AvoidSingularityTermInfo (problem_description.cpp:1900-1939): one object per step first..last on the smallest
+    singular value of `link`'s geometric Jacobian; an ABS cost (role COST) or an INEQ constraint (role CNT)."""
+    t = Term()
+    t.kind, t.role, t.first_step, t.last_step = TERM_AVOID_SINGULARITY, role, first, last
+    t.link, t.target_slot = link, -1
+    t.coeffs[0] = coeff
+    t.lambda_ = lam
     return t
 
 

@@ -164,3 +164,26 @@ def rot_to_wxyz(R):
 def sphere_centers(robot, q):
     fr = fk_numpy(robot, q)
     return np.array([fr[s.segment][0] @ np.array(list(s.center)) + fr[s.segment][1] for s in robot["spheres"]])
+
+
+def jacobian_numpy(robot, q, link):
+    """6 x n_dof geometric Jacobian of segment `link`'s origin in the scene root (linear rows, then angular; a zero
+    column for a joint that does not move the link): the matrix of the avoid_singularity term."""
+    fr = fk_numpy(robot, q)
+    segs = robot["segments"]
+    J = np.zeros((6, robot["n_dof"]))
+    pe = fr[link][1]
+    s = link
+    while s >= 0:
+        g = segs[s]
+        if g.joint_type != JOINT_FIXED:
+            R, o = fr[s]
+            a = R @ np.array(list(g.axis))
+            J[:, g.q_index] = np.r_[np.cross(a, pe - o), a] if g.joint_type == JOINT_REVOLUTE else np.r_[a, 0, 0, 0]
+        s = g.parent
+    return J
+
+
+def smallest_singular_value(robot, q, link):
+    """The smallest singular value of jacobian_numpy (thin SVD: the smallest of min(6, n_dof))."""
+    return float(np.linalg.svd(jacobian_numpy(robot, q, link), compute_uv=False)[-1])
