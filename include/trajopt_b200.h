@@ -219,6 +219,9 @@ typedef struct tb200_problem_desc {
    * The best seed of every group is selected on the device (tb200_fetch_group_results). */
   int32_t group_size;
   int32_t group_stop;
+  /* Per-trajectory optimizer parameters (not in the reference; DESIGN.md section 4.1): [batch] rows, trajectory b runs
+   * under row b (every field, max_time against the one clock of the batch); NULL: `sqp` for every trajectory. */
+  const tb200_sqp_params* sqp_per_traj;
 } tb200_problem_desc;
 
 /* Caller-owned result buffers = sco::OptResults per trajectory (optimizers.hpp:40-59).
@@ -310,8 +313,12 @@ void tb200_problem_destroy(tb200_problem* p);
 int tb200_problem_layout(const tb200_problem* p, tb200_layout* out);
 
 /* Replace the optimizer parameters of an existing problem (what `opt.getParameters() = ...` does on a
- * sco::BasicTrustRegionSQP, optimizers.hpp:92-135, 365-366).  Takes effect at the next solve. */
+ * sco::BasicTrustRegionSQP, optimizers.hpp:92-135, 365-366), for every trajectory: a per-trajectory table is dropped.
+ * Takes effect at the next solve. */
 int tb200_problem_set_sqp_params(tb200_problem* p, const tb200_sqp_params* params);
+/* Per-trajectory optimizer parameters: rows [batch], trajectory b runs under rows[b] (as tb200_problem_desc.sqp_per_traj);
+ * NULL drops the table, and every trajectory runs under the uniform parameters again.  Takes effect at the next solve. */
+int tb200_problem_set_sqp_params_per_traj(tb200_problem* p, const tb200_sqp_params* rows);
 
 /* Replace the per-trajectory inputs without rebuilding (same shapes). Host pointers. */
 int tb200_problem_set_inputs(tb200_problem* p, const double* init_traj, const double* cart_targets,

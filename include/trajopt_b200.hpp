@@ -357,6 +357,39 @@ struct FlatProblem {
   std::shared_ptr<const RobotModel> kin;  // pci.kin (WriteCallback's FK)
 };
 
+// The C ABI's form of one set of optimizer parameters (log_results / log_dir stay on the host).
+inline tb200_sqp_params ToSqpParams(const sco::BasicTrustRegionSQPParameters& p) {
+  tb200_sqp_params s{};
+  s.improve_ratio_threshold = p.improve_ratio_threshold;
+  s.min_trust_box_size = p.min_trust_box_size;
+  s.min_approx_improve = p.min_approx_improve;
+  s.min_approx_improve_frac = p.min_approx_improve_frac;
+  s.max_iter = p.max_iter;
+  s.max_qp_solver_failures = p.max_qp_solver_failures;
+  s.trust_shrink_ratio = p.trust_shrink_ratio;
+  s.trust_expand_ratio = p.trust_expand_ratio;
+  s.cnt_tolerance = p.cnt_tolerance;
+  s.max_merit_coeff_increases = p.max_merit_coeff_increases;
+  s.merit_coeff_increase_ratio = p.merit_coeff_increase_ratio;
+  s.initial_merit_error_coeff = p.initial_merit_error_coeff;
+  s.trust_box_size = p.trust_box_size;
+  s.inflate_constraints_individually = p.inflate_constraints_individually ? 1 : 0;
+  s.reserved = 0;
+  s.max_time = p.max_time;
+  return s;
+}
+// The per-trajectory table (tb200_problem_set_sqp_params_per_traj) of a batch of `batch` problems, row b from params[b];
+// throws std::invalid_argument unless there is exactly one entry per problem.
+inline std::vector<tb200_sqp_params> SqpParamRows(int batch, const std::vector<sco::BasicTrustRegionSQPParameters>& params) {
+  if (params.size() != static_cast<size_t>(batch))
+    throw std::invalid_argument("per-problem optimizer parameters: " + std::to_string(params.size()) +
+                                " entries for a batch of " + std::to_string(batch));
+  std::vector<tb200_sqp_params> rows;
+  rows.reserve(params.size());
+  for (const sco::BasicTrustRegionSQPParameters& p : params) rows.push_back(ToSqpParams(p));
+  return rows;
+}
+
 // The part of ConstructProblem (problem_description.cpp:410-542) that does not need the device: checks, initial
 // trajectory (InitInfo, :330-408), term hatching into the POD description (cost_infos first, then cnt_infos).
 inline std::shared_ptr<FlatProblem> FlattenProblem(const ProblemConstructionInfo& pci) {
@@ -459,23 +492,7 @@ inline std::shared_ptr<FlatProblem> FlattenProblem(const ProblemConstructionInfo
   d.obstacles_per_traj = pci.obstacles_per_problem ? 1 : 0;
   d.obstacles = fp->obstacles.empty() ? nullptr : fp->obstacles.data();
   tb200_default_qp_settings(&d.qp);  // OSQPModelConfig::setDefaultOSQPSettings, osqp_interface.cpp:78-90
-  const sco::BasicTrustRegionSQPParameters& p = pci.opt_info;
-  d.sqp.improve_ratio_threshold = p.improve_ratio_threshold;
-  d.sqp.min_trust_box_size = p.min_trust_box_size;
-  d.sqp.min_approx_improve = p.min_approx_improve;
-  d.sqp.min_approx_improve_frac = p.min_approx_improve_frac;
-  d.sqp.max_iter = p.max_iter;
-  d.sqp.max_qp_solver_failures = p.max_qp_solver_failures;
-  d.sqp.trust_shrink_ratio = p.trust_shrink_ratio;
-  d.sqp.trust_expand_ratio = p.trust_expand_ratio;
-  d.sqp.cnt_tolerance = p.cnt_tolerance;
-  d.sqp.max_merit_coeff_increases = p.max_merit_coeff_increases;
-  d.sqp.merit_coeff_increase_ratio = p.merit_coeff_increase_ratio;
-  d.sqp.initial_merit_error_coeff = p.initial_merit_error_coeff;
-  d.sqp.trust_box_size = p.trust_box_size;
-  d.sqp.inflate_constraints_individually = p.inflate_constraints_individually ? 1 : 0;
-  d.sqp.reserved = 0;
-  d.sqp.max_time = p.max_time;
+  d.sqp = ToSqpParams(pci.opt_info);
   d.group_size = pci.seeds_per_problem;
   d.group_stop = pci.stop_seeds_on_converged ? 1 : 0;
   return fp;
@@ -517,8 +534,20 @@ inline TrajOptProb::Ptr ConstructProblem(const ProblemConstructionInfo& pci, int
 // BasicTrustRegionSQP::optimize() for every problem of the batch (optimizers.cpp:699-991) with the given parameters: what
 // `sco::BasicTrustRegionSQP opt(prob); opt.getParameters() = params; opt.initialize(...); opt.optimize(); opt.results()`
 // returns, per problem.
+namespace detail {
+// Sets the optimizer parameters of the next solve: one row for every problem, or one row per problem (B > 1).
+inline void setSqpParams(TrajOptProb& prob, const std::vector<tb200_sqp_params>& rows) {
+  const int rc = rows.size() == 1 ? tb200_problem_set_sqp_params(prob.handle(), rows.data())
+                                  : tb200_problem_set_sqp_params_per_traj(prob.handle(), rows.data());
+  if (rc != TB200_OK) throw std::runtime_error(tb200_last_error());
+}
+inline std::vector<sco::OptResults> solveBatch(TrajOptProb& prob);
+}  // namespace detail
 inline std::vector<sco::OptResults> OptimizeWithParams(TrajOptProb& prob, const tb200_sqp_params& params) {
-  if (tb200_problem_set_sqp_params(prob.handle(), &params) != TB200_OK) throw std::runtime_error(tb200_last_error());
+  detail::setSqpParams(prob, {params});
+  return detail::solveBatch(prob);
+}
+inline std::vector<sco::OptResults> detail::solveBatch(TrajOptProb& prob) {
   const size_t B = prob.GetBatch(), N = static_cast<size_t>(prob.GetNumSteps()) * prob.GetNumDOF();
   const size_t nc = prob.getNumCosts(), nk = prob.getNumConstraints();
   DblVec x(B * N), total(B), cv(B * (nc ? nc : 1)), kv(B * (nk ? nk : 1));
@@ -740,27 +769,53 @@ inline void WriteLogResults(const SqpLog& L, std::size_t b, const std::string& d
 // and the host a copy of it: at configs[2] (batch 1024, 30 x 7 variables, 16 objects) 2560 bytes a record, 0.66 GB for
 // the default 251 records.  When a problem needed more, the batch is solved once more with exactly the capacity the log
 // counted (the solve is deterministic), unless allow_truncated asks for the prefix.
+// With per-problem parameters the default capacity is the largest of those products, and log_results / log_dir are read
+// per problem.
 namespace detail {
-inline std::vector<sco::OptResults> optimizeLogged(TrajOptProb& prob, const tb200_sqp_params& params,
-                                                   const std::vector<Callback>& callbacks, bool log_results,
-                                                   int log_capacity, bool allow_truncated);
+// rows: one for every problem or one per problem (setSqpParams); log_dirs: per problem, the directory its log_results
+// files go to ("": none), or empty for no files at all
+inline std::vector<sco::OptResults> optimizeLogged(TrajOptProb& prob, const std::vector<tb200_sqp_params>& rows,
+                                                   const std::vector<Callback>& callbacks,
+                                                   const std::vector<std::string>& log_dirs, int log_capacity,
+                                                   bool allow_truncated);
+// log_dir/<problem> for every problem when log_results, else none
+inline std::vector<std::string> logDirs(const TrajOptProb& prob, bool log_results, const std::string& log_dir) {
+  std::vector<std::string> dirs;
+  if (log_results)
+    for (int b = 0; b < prob.GetBatch(); ++b) dirs.push_back(log_dir + "/" + std::to_string(b));
+  return dirs;
 }
+inline std::vector<std::string> logDirs(const std::vector<sco::BasicTrustRegionSQPParameters>& params) {
+  std::vector<std::string> dirs;
+  bool any = false;
+  for (size_t b = 0; b < params.size(); ++b) {
+    dirs.push_back(params[b].log_results ? params[b].log_dir + "/" + std::to_string(b) : std::string());
+    any = any || params[b].log_results;
+  }
+  return any ? dirs : std::vector<std::string>();
+}
+}  // namespace detail
 inline std::vector<sco::OptResults> OptimizeWithParams(TrajOptProb& prob, const tb200_sqp_params& params,
                                                        const std::vector<Callback>& callbacks, int log_capacity = 0,
                                                        bool allow_truncated = false) {
-  return detail::optimizeLogged(prob, params, callbacks, prob.flat().log_results, log_capacity, allow_truncated);
+  return detail::optimizeLogged(prob, {params}, callbacks, detail::logDirs(prob, prob.flat().log_results, prob.flat().log_dir),
+                                log_capacity, allow_truncated);
 }
-inline std::vector<sco::OptResults> detail::optimizeLogged(TrajOptProb& prob, const tb200_sqp_params& params,
-                                                           const std::vector<Callback>& callbacks, bool log_results,
-                                                           int log_capacity, bool allow_truncated) {
-  int cap = log_capacity > 0 ? log_capacity
-                             : 1 + std::max(params.max_iter, 1) * static_cast<int>(std::ceil(std::max(params.max_merit_coeff_increases, 1.0)));
+inline std::vector<sco::OptResults> detail::optimizeLogged(TrajOptProb& prob, const std::vector<tb200_sqp_params>& rows,
+                                                           const std::vector<Callback>& callbacks,
+                                                           const std::vector<std::string>& log_dirs, int log_capacity,
+                                                           bool allow_truncated) {
+  int cap = log_capacity;
+  if (cap <= 0)
+    for (const tb200_sqp_params& p : rows)
+      cap = std::max(cap, 1 + std::max(p.max_iter, 1) * static_cast<int>(std::ceil(std::max(p.max_merit_coeff_increases, 1.0))));
   std::vector<sco::OptResults> out;
   SqpLog L;
   try {
     for (;;) {
       if (tb200_problem_set_sqp_log(prob.handle(), cap, 1) != TB200_OK) throw std::runtime_error(tb200_last_error());
-      out = OptimizeWithParams(prob, params);
+      setSqpParams(prob, rows);
+      out = solveBatch(prob);
       L = FetchSqpLog(prob, cap, true);
       int need = 0;
       for (int b = 0; b < L.B; ++b) need = std::max(need, L.n_records[b] + L.n_dropped[b]);
@@ -773,13 +828,13 @@ inline std::vector<sco::OptResults> detail::optimizeLogged(TrajOptProb& prob, co
   }
   tb200_problem_set_sqp_log(prob.handle(), 0, 0);
   std::vector<std::string> var_names, cost_names, cnt_names;
-  if (log_results) {
+  if (!log_dirs.empty()) {
     var_names = VarNames(prob.GetNumSteps(), prob.GetNumDOF());
     ObjectNames(prob, cost_names, cnt_names);
   }
   for (size_t b = 0; b < out.size(); ++b) {
     ReplayCallbacks(&prob, L, b, out[b], callbacks, allow_truncated);
-    if (log_results) WriteLogResults(L, b, prob.flat().log_dir + "/" + std::to_string(b), var_names, cost_names, cnt_names);
+    if (!log_dirs.empty() && !log_dirs[b].empty()) WriteLogResults(L, b, log_dirs[b], var_names, cost_names, cnt_names);
   }
   return out;
 }
@@ -796,11 +851,32 @@ inline std::vector<sco::OptResults> OptimizeProblem(TrajOptProb& prob, const std
   p.min_approx_improve_frac = .001;
   p.improve_ratio_threshold = .2;
   p.initial_merit_error_coeff = 20;
-  return detail::optimizeLogged(prob, p, callbacks, false, 0, false);
+  return detail::optimizeLogged(prob, {p}, callbacks, {}, 0, false);
 }
 inline std::vector<sco::OptResults> OptimizeWithParams(TrajOptProb& prob) {
-  if (prob.flat().log_results) return detail::optimizeLogged(prob, prob.sqpParams(), {}, true, 0, false);
+  if (prob.flat().log_results)
+    return detail::optimizeLogged(prob, {prob.sqpParams()}, {}, detail::logDirs(prob, true, prob.flat().log_dir), 0, false);
   return OptimizeWithParams(prob, prob.sqpParams());
+}
+
+// Per-problem parameters (not in the reference; DESIGN.md section 4.1): problem b of the batch runs under params[b], with
+// exactly the results a batch solved under params[b] alone would give it.  One entry per problem of the batch, else
+// std::invalid_argument.  With callbacks, or when some entry has log_results, the batch is solved with the SQP log as in
+// the overload with callbacks; problem b's files go to params[b].log_dir/<b>.
+inline std::vector<sco::OptResults> OptimizeWithParams(TrajOptProb& prob,
+                                                       const std::vector<sco::BasicTrustRegionSQPParameters>& params,
+                                                       const std::vector<Callback>& callbacks, int log_capacity = 0,
+                                                       bool allow_truncated = false) {
+  return detail::optimizeLogged(prob, SqpParamRows(prob.GetBatch(), params), callbacks, detail::logDirs(params), log_capacity,
+                                allow_truncated);
+}
+inline std::vector<sco::OptResults> OptimizeWithParams(TrajOptProb& prob,
+                                                       const std::vector<sco::BasicTrustRegionSQPParameters>& params) {
+  const std::vector<tb200_sqp_params> rows = SqpParamRows(prob.GetBatch(), params);
+  const std::vector<std::string> dirs = detail::logDirs(params);
+  if (!dirs.empty()) return detail::optimizeLogged(prob, rows, {}, dirs, 0, false);
+  detail::setSqpParams(prob, rows);
+  return detail::solveBatch(prob);
 }
 
 // The frames of every link of a RobotModel at joint values q: the arithmetic of the test oracle's Robot::fk (origin
@@ -933,8 +1009,19 @@ struct MultiStartResult {
 // Every problem of a multi-start batch, with the given parameters: the seeds are solved together (siblings stopped on the
 // device when pci.stop_seeds_on_converged) and the best seed of each problem is selected on the device by the key of
 // tb200_group_results (converged first, then the smallest constraint violation, then total cost, then index).
+namespace detail {
+inline std::vector<MultiStartResult> selectSeeds(TrajOptProb& prob, const std::vector<sco::OptResults>& seeds);
+}
 inline std::vector<MultiStartResult> OptimizeProblemMultiStart(TrajOptProb& prob, const tb200_sqp_params& params) {
-  const std::vector<sco::OptResults> seeds = OptimizeWithParams(prob, params);
+  return detail::selectSeeds(prob, OptimizeWithParams(prob, params));
+}
+// ... with per-seed parameters (a parameter portfolio: the seeds of a problem may differ in their parameters as well as in
+// their initial trajectory); params[b] for batch index b, as in OptimizeWithParams
+inline std::vector<MultiStartResult> OptimizeProblemMultiStart(TrajOptProb& prob,
+                                                              const std::vector<sco::BasicTrustRegionSQPParameters>& params) {
+  return detail::selectSeeds(prob, OptimizeWithParams(prob, params));
+}
+inline std::vector<MultiStartResult> detail::selectSeeds(TrajOptProb& prob, const std::vector<sco::OptResults>& seeds) {
   const int G = prob.GetSeedsPerProblem(), NG = prob.GetBatch() / G;
   std::vector<int32_t> best(NG);
   tb200_group_results g{};

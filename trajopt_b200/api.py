@@ -58,8 +58,16 @@ class Problem:
         self._check(self.lib.tb200_problem_set_inputs(self.handle, *[None if a is None else _dp(a) for a in keep]))
 
     def set_sqp_params(self, sqp):
-        """Replace the optimizer parameters (a capi.SqpParams, e.g. with a new max_time) for the next solves."""
-        self._check(self.lib.tb200_problem_set_sqp_params(self.handle, C.byref(sqp)))
+        """Replace the optimizer parameters for the next solves: one capi.SqpParams (e.g. with a new max_time) for every
+        trajectory, or a sequence of B of them, row b for trajectory b (None: drop such a table; the last uniform
+        parameters apply again)."""
+        if sqp is None:
+            self._check(self.lib.tb200_problem_set_sqp_params_per_traj(self.handle, None))
+        elif isinstance(sqp, capi.SqpParams):
+            self._check(self.lib.tb200_problem_set_sqp_params(self.handle, C.byref(sqp)))
+        else:
+            rows = capi.sqp_table(sqp, self.desc.B)
+            self._check(self.lib.tb200_problem_set_sqp_params_per_traj(self.handle, rows))
 
     def set_groups(self, group_size, group_stop=0):
         """Multi-start: trajectories [g*G, (g+1)*G) are G seeds of problem g (G = 0 or 1: no groups); group_stop 1

@@ -79,7 +79,7 @@ class ProblemDescC(C.Structure):
                 ("n_fixed_dofs", C.c_int32), ("n_cart_targets", C.c_int32), ("fixed_dofs", _i32_p),
                 ("init_traj", _dbl_p), ("cart_targets", _dbl_p), ("n_obstacles", C.c_int32),
                 ("obstacles_per_traj", C.c_int32), ("obstacles", _dbl_p), ("sqp", SqpParams), ("qp", QpSettings),
-                ("group_size", C.c_int32), ("group_stop", C.c_int32)]
+                ("group_size", C.c_int32), ("group_stop", C.c_int32), ("sqp_per_traj", C.POINTER(SqpParams))]
 
 
 class QpGeneral(C.Structure):
@@ -172,6 +172,14 @@ def default_qp_settings():
     return s
 
 
+def sqp_table(rows, B):
+    """A ctypes array of B SqpParams (the per-trajectory table of tb200_problem_desc.sqp_per_traj) from a sequence."""
+    rows = list(rows)
+    if len(rows) != B:
+        raise ValueError(f"{len(rows)} parameter rows for a batch of {B}")
+    return (SqpParams * B)(*rows)
+
+
 def _dp(a):
     return a.ctypes.data_as(_dbl_p) if a is not None else None
 
@@ -184,9 +192,10 @@ class ProblemDesc:
     """Python-side owner of a tb200_problem_desc: keeps every buffer alive."""
 
     def __init__(self, robot, n_steps, terms, init_traj, fixed_timesteps=(), fixed_dofs=(), cart_targets=None,
-                 obstacles=None, obstacles_per_traj=True, sqp=None, qp=None, group_size=0, group_stop=0):
+                 obstacles=None, obstacles_per_traj=True, sqp=None, qp=None, group_size=0, group_stop=0, sqp_per_traj=None):
         """group_size G >= 2: trajectories [g*G, (g+1)*G) are G seeds of problem g; group_stop 1: the siblings of a seed
-        that converges stop at their next SQP iteration top (include/trajopt_b200.h)."""
+        that converges stop at their next SQP iteration top (include/trajopt_b200.h).  sqp_per_traj: B SqpParams, the
+        parameters trajectory b runs under (None: `sqp` for every trajectory)."""
         self.robot_spec = robot
         init_traj = np.ascontiguousarray(init_traj, dtype=np.float64)
         assert init_traj.ndim == 3 and init_traj.shape[1] == n_steps and init_traj.shape[2] == robot["n_dof"]
@@ -229,6 +238,10 @@ class ProblemDesc:
         d.sqp = sqp if sqp is not None else default_sqp_params()
         d.qp = qp if qp is not None else default_qp_settings()
         d.group_size, d.group_stop = group_size, group_stop
+        self.sqp_per_traj = None
+        if sqp_per_traj is not None:
+            self.sqp_per_traj = sqp_table(sqp_per_traj, self.B)
+            d.sqp_per_traj = self.sqp_per_traj
         self.c = d
 
     def slice(self, b0, b1):
@@ -243,7 +256,8 @@ class ProblemDesc:
                            obstacles=None if self.obstacles is None else
                            (self.obstacles[b0:b1] if self.c.obstacles_per_traj else self.obstacles),
                            obstacles_per_traj=bool(self.c.obstacles_per_traj), sqp=self.c.sqp, qp=self.c.qp,
-                           group_size=self.c.group_size, group_stop=self.c.group_stop)
+                           group_size=self.c.group_size, group_stop=self.c.group_stop,
+                           sqp_per_traj=None if self.sqp_per_traj is None else self.sqp_per_traj[b0:b1])
 
 
 def alloc_results(B, T, D, n_costs, n_cnts):
@@ -297,6 +311,7 @@ def load_library():
     lib.tb200_last_timing.argtypes = [C.c_void_p, C.POINTER(Timing)]
     lib.tb200_default_sqp_params.argtypes = [C.POINTER(SqpParams)]
     lib.tb200_problem_set_sqp_params.argtypes = [C.c_void_p, C.POINTER(SqpParams)]
+    lib.tb200_problem_set_sqp_params_per_traj.argtypes = [C.c_void_p, C.POINTER(SqpParams)]
     lib.tb200_default_qp_settings.argtypes = [C.POINTER(QpSettings)]
     lib.tb200_problem_set_groups.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
     lib.tb200_fetch_group_results.argtypes = [C.c_void_p, C.POINTER(GroupResults)]
@@ -315,5 +330,5 @@ EXPORTED_SYMBOLS = [
     "tb200_qp_solve_batch", "tb200_last_qp_polish", "tb200_last_timing",
     "tb200_qp_solve_general", "tb200_qp_general_last_error", "tb200_osqp_order_qp_settings", "tb200_problem_set_sqp_params",
     "tb200_problem_set_groups", "tb200_fetch_group_results", "tb200_check_trajectories",
-    "tb200_problem_set_sqp_log", "tb200_fetch_sqp_log", "tb200_problem_objects",
+    "tb200_problem_set_sqp_log", "tb200_fetch_sqp_log", "tb200_problem_objects", "tb200_problem_set_sqp_params_per_traj",
 ]

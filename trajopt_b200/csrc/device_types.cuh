@@ -165,15 +165,14 @@ struct DevProblem {
   double* dbg;                 // [B][16] solver diagnostics of the last QP (residuals, polish residuals, rho, c)
   int* sched_state;            // [B] persistent SQP kernel: 0 ready, 1 running, 2 finished
   unsigned long long* sched_timers;  // [4] ns in QP steps, ns in evaluation steps, evaluation steps, claims
-  unsigned long long* clock_start;   // [1] %globaltimer ns at the start of the solve: the clock of sqp.max_time
+  unsigned long long* clock_start;   // [1] %globaltimer ns at the start of the solve: the clock of every max_time
   int* sqp_top;                // [B] 1: the next QP of the trajectory begins a new SQP iteration (the time-limit check)
-  int* ended_by;               // [B] what ended the trajectory: 0 its own SQP, 1 sqp.max_time, 2 its group (group_stop)
+  int* ended_by;               // [B] what ended the trajectory: 0 its own SQP, 1 its max_time, 2 its group (group_stop)
   int* group_done;             // [B / group_size] 1: a seed of the group ended OPT_CONVERGED by its own SQP (group_stop)
   int group_size;              // seeds per problem: trajectories [g*G, (g+1)*G) are group g; 1 without groups
   int group_stop;              // 1: the siblings of a converged seed end at their next SQP iteration top (only with G > 1)
   QpSettings qp;
   int qp_fast_passes;  // 1: short trajectories take the fused termination check and polish_passes (qp_cta_kernel.cuh)
-  SqpParams sqp;
 };
 
 // Record layout of the SQP iteration log: a header of kLogHeader doubles, then n_cnts merit coefficients, the model values

@@ -100,6 +100,10 @@ struct EvalExtra {
   // AvoidSingularity objects (one per step; coeff: the term's coefficient, margin: its lambda)
   const DevObj* sing_objs;
   int n_sing_objs, pad_sing;
+  // Optimizer parameters, [B]: trajectory b runs under sqp[b] (tb200_problem_set_sqp_params / _per_traj fill every row).
+  // sqp_timed: some row has a time limit (max_time < DBL_MAX); the clock check at the iteration top is one uniform branch.
+  const SqpParams* sqp;
+  int sqp_timed, pad_sqp;
 };
 
 #ifdef TB200_EVAL_PROFILE
@@ -1094,7 +1098,7 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
 
   // ---- trust-region / penalty state machine (thread 0), optimizers.cpp:811-968 ----------------------
   if (tid == 0) {
-    const SqpParams& sp = p.sqp;
+    const SqpParams& sp = ex.sqp[b];  // (this trajectory's row)
     double* mu = p.merit_coeffs + static_cast<size_t>(b) * p.n_cnts;
     double* cv = p.cost_vals + static_cast<size_t>(b) * p.n_costs;
     double* kv = p.cnt_viols + static_cast<size_t>(b) * p.n_cnts;

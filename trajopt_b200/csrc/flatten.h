@@ -44,6 +44,7 @@ struct FlatProblem {
   bool has_vel = false, has_cast = false;
   int cast_cap = 0;  // active contacts (rows) a step pair of the continuous evaluator can hold
   int n_joint_objs = 0, joint_obj_idx[8] = {};  // positions of the joint-space objects in the (costs, cnts) list
+  std::vector<SqpParams> sqp_rows;  // [B] optimizer parameters of trajectory b (sqp_per_traj[b], or sqp for every b)
 };
 
 namespace flat {
@@ -59,6 +60,22 @@ inline int check_groups(int B, int group_size, int group_stop, std::string& msg)
     return refuse(msg, TB200_ERR_INVALID, "batch " + std::to_string(B) + " is not a multiple of group_size " + std::to_string(group_size));
   if (group_stop != 0 && group_stop != 1) return refuse(msg, TB200_ERR_INVALID, "group_stop must be 0 or 1");
   return TB200_OK;
+}
+
+inline SqpParams sqp_params(const tb200_sqp_params& s) {
+  return SqpParams{s.improve_ratio_threshold, s.min_trust_box_size, s.min_approx_improve, s.min_approx_improve_frac,
+                   s.trust_shrink_ratio, s.trust_expand_ratio, s.cnt_tolerance, s.max_merit_coeff_increases,
+                   s.merit_coeff_increase_ratio, s.initial_merit_error_coeff, s.trust_box_size, s.max_iter,
+                   s.max_qp_solver_failures, s.inflate_constraints_individually, 0, s.max_time};
+}
+
+// The parameters every trajectory of a batch of B runs under: rows[b] of a per-trajectory table, or `uniform` for every
+// trajectory when there is none (rows NULL).
+inline std::vector<SqpParams> sqp_rows(int B, const tb200_sqp_params& uniform, const tb200_sqp_params* rows) {
+  std::vector<SqpParams> out(static_cast<size_t>(B), sqp_params(uniform));
+  if (rows)
+    for (int b = 0; b < B; ++b) out[b] = sqp_params(rows[b]);
+  return out;
 }
 
 inline void quat_to_rot(const double* q, double* R) {
@@ -428,6 +445,7 @@ inline int flatten(const tb200_problem_desc& d, FlatProblem& F, std::string& msg
     }
   if (F.n_joint_objs > 8) return flat::refuse(msg, TB200_ERR_UNSUPPORTED, "more than 8 joint-space cost/constraint objects");
   if (d.n_obstacles > 64) return flat::refuse(msg, TB200_ERR_UNSUPPORTED, "more than 64 obstacle spheres per trajectory");
+  F.sqp_rows = flat::sqp_rows(d.batch, d.sqp, d.sqp_per_traj);
   return TB200_OK;
 }
 

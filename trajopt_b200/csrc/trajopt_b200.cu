@@ -41,13 +41,6 @@ void setGroups(DevProblem& dp, int group_size, int group_stop) {
   dp.group_size = std::max(group_size, 1);
   dp.group_stop = dp.group_size > 1 ? group_stop : 0;
 }
-
-SqpParams sqpParams(const tb200_sqp_params& s) {
-  return SqpParams{s.improve_ratio_threshold, s.min_trust_box_size, s.min_approx_improve, s.min_approx_improve_frac,
-                   s.trust_shrink_ratio, s.trust_expand_ratio, s.cnt_tolerance, s.max_merit_coeff_increases,
-                   s.merit_coeff_increase_ratio, s.initial_merit_error_coeff, s.trust_box_size, s.max_iter,
-                   s.max_qp_solver_failures, s.inflate_constraints_individually, 0, s.max_time};
-}
 }  // namespace
 
 struct tb200_problem {
@@ -68,6 +61,10 @@ struct tb200_problem {
   DevBuf<int> log_len, log_dropped;
   bool pair_rows = false;  // QP rows span two waypoints (CartVel, continuous collision): 2*D coefficients per row
   bool sing = false;       // AvoidSingularity objects: the kernel instances with the term (SING = 1)
+  // optimizer parameters: the uniform ones (tb200_problem_set_sqp_params), and the [B] rows the kernels read (EvalExtra::sqp),
+  // the uniform ones in every row unless a per-trajectory table was given
+  tb200_sqp_params sqp_uniform{};
+  DevBuf<SqpParams> sqp_rows;
   // device storage
   DevBuf<DevSegment> segs;
   DevBuf<DevSphere> spheres;
@@ -152,7 +149,7 @@ int planLayout(const tb200_problem_desc& d, const FlatProblem& F, tb200_problem&
                      d.qp.delta, d.qp.adaptive_rho_tolerance, d.qp.max_iter, d.qp.scaling, d.qp.check_termination,
                      d.qp.adaptive_rho, d.qp.adaptive_rho_interval, d.qp.polishing, d.qp.polish_refine_iter,
                      d.qp.warm_starting, d.qp.early_polish_every, d.qp.early_polish_from};
-  dp.sqp = sqpParams(d.sqp);
+  P.sqp_uniform = d.sqp;
   setGroups(dp, d.group_size, d.group_stop);
   EvalExtra& ex = P.ex;
   ex.n_cart_objs = static_cast<int>(F.cart_objs.size());
@@ -270,6 +267,7 @@ int allocate(const tb200_problem_desc& d, FlatProblem& F, tb200_problem& P) {
   dp.qp_done = zeros(P.qp_done, B); dp.ws_rho = zeros(P.ws_rho, B); dp.ws_meta = zeros(P.ws_meta, B * 8);
   dp.lvs_overflow = zeros(P.lvs_overflow, B);
   ex.work_counter = zeros(P.work_counter, 1);
+  ex.sqp = zeros(P.sqp_rows, B);
   // contact lists of the continuous collision evaluator: one per resident warp of the largest launch (4 doubles a contact)
   ex.cast_scratch = zeros(P.cast_scratch, ex.cast ? static_cast<size_t>(std::max(P.eval_grid, std::min(P.B, P.n_sm))) *
                                                         (kEvalThreads / 32) * 4 * ex.cast_cap : 0);
@@ -291,7 +289,19 @@ int allocate(const tb200_problem_desc& d, FlatProblem& F, tb200_problem& P) {
   zeros(P.g_best, B); zeros(P.g_status, B); zeros(P.g_n_converged, B); zeros(P.g_total_cost, B); zeros(P.g_x, B * N);
   zeros(P.x_tmp, B * N); zeros(P.trust_tmp, B); zeros(P.tmp_iters, B); zeros(P.tmp_polish, B);
   if (e != cudaSuccess) return fail(TB200_ERR_CUDA, std::string("device buffers of the problem: ") + cudaGetErrorString(e));
+  // the zero fills (cudaMemset, asynchronous on the legacy stream) end before the uploads on the solver's non-blocking
+  // stream, which does not wait for them
+  CK(cudaDeviceSynchronize());
   P.obj_src = std::move(F.obj_src);
+  return TB200_OK;
+}
+
+// Uploads the optimizer parameters of the next solves, row b for trajectory b, and whether any row has a time limit.
+int uploadSqpRows(tb200_problem& P, const std::vector<SqpParams>& rows) {
+  CK(cudaSetDevice(P.device));
+  CK(cudaMemcpyAsync(P.sqp_rows.p, rows.data(), rows.size() * sizeof(SqpParams), cudaMemcpyHostToDevice, P.stream));
+  CK(cudaStreamSynchronize(P.stream));
+  P.ex.sqp_timed = std::any_of(rows.begin(), rows.end(), [](const SqpParams& r) { return r.max_time < kNoTimeLimit; });
   return TB200_OK;
 }
 
@@ -353,6 +363,7 @@ int tb200_problem_create(const tb200_problem_desc* d, int device, tb200_problem*
   if (int rc = planLayout(*d, F, *P)) return rc;
   if (int rc = setupDevice(*P, device)) return rc;
   if (int rc = allocate(*d, F, *P)) return rc;
+  if (int rc = uploadSqpRows(*P, F.sqp_rows)) return rc;
   if (int rc = tb200_problem_set_inputs(P.get(), d->init_traj, d->cart_targets, d->obstacles)) return rc;
   *out = P.release();
   return TB200_OK;
@@ -369,8 +380,13 @@ int tb200_problem_layout(const tb200_problem* p, tb200_layout* out) {
 
 int tb200_problem_set_sqp_params(tb200_problem* P, const tb200_sqp_params* s) {
   if (!P || !s) return fail(TB200_ERR_INVALID, "null argument");
-  P->dp.sqp = sqpParams(*s);
-  return TB200_OK;
+  P->sqp_uniform = *s;
+  return uploadSqpRows(*P, flat::sqp_rows(P->B, *s, nullptr));
+}
+
+int tb200_problem_set_sqp_params_per_traj(tb200_problem* P, const tb200_sqp_params* rows) {
+  if (!P) return fail(TB200_ERR_INVALID, "null problem");
+  return uploadSqpRows(*P, flat::sqp_rows(P->B, P->sqp_uniform, rows));
 }
 
 int tb200_problem_set_groups(tb200_problem* P, int32_t group_size, int32_t group_stop) {
@@ -402,7 +418,7 @@ int tb200_problem_set_inputs(tb200_problem* P, const double* init_traj, const do
 }
 
 namespace {
-__global__ void reset_state_kernel(DevProblem p, int* log_len, int* log_dropped) {
+__global__ void reset_state_kernel(DevProblem p, const SqpParams* sqp, int* log_len, int* log_dropped) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b == 0) {
     p.active_count[0] = p.B;
@@ -420,8 +436,8 @@ __global__ void reset_state_kernel(DevProblem p, int* log_len, int* log_dropped)
   p.n_qp_solves[b] = 0;
   p.n_func_evals[b] = 0;
   p.n_admm_iters[b] = 0;
-  p.trust[b] = p.sqp.trust_box_size;
-  for (int c = 0; c < p.n_cnts; ++c) p.merit_coeffs[static_cast<size_t>(b) * p.n_cnts + c] = p.sqp.initial_merit_error_coeff;
+  p.trust[b] = sqp[b].trust_box_size;
+  for (int c = 0; c < p.n_cnts; ++c) p.merit_coeffs[static_cast<size_t>(b) * p.n_cnts + c] = sqp[b].initial_merit_error_coeff;
   for (int k = 0; k < 8; ++k) p.ws_meta[b * 8 + k] = 0;
   p.qp_done[b] = 0;
   p.lvs_overflow[b] = 0;
@@ -578,7 +594,7 @@ int tb200_solve_batch_resident(tb200_problem* P) {
   if (int rc = applyLogSetting(P)) return rc;
   cudaEvent_t e_begin = getEvent(P, 0), e_end = getEvent(P, 1), e_init0 = getEvent(P, 2), e_init1 = getEvent(P, 3);
   CK(cudaEventRecord(e_begin, st));
-  reset_state_kernel<<<(dp.B + 127) / 128, 128, 0, st>>>(dp, P->ex.log_len, P->ex.log_dropped);
+  reset_state_kernel<<<(dp.B + 127) / 128, 128, 0, st>>>(dp, P->ex.sqp, P->ex.log_len, P->ex.log_dropped);
   if (dp.qp_paths) CK(cudaMemsetAsync(dp.qp_paths, 0, dp.B * sizeof(int), st));
   // the initial evaluation + convexification of every trajectory: one CTA per trajectory (optimizers.cpp:761-783)
   CK(cudaEventRecord(e_init0, st));

@@ -203,7 +203,8 @@ def with_seeds(desc, n_seeds, rng, spread, group_stop=0):
     per_traj = bool(d.c.obstacles_per_traj)
     return ProblemDesc(d.robot_spec, d.T, d.terms, init, fixed_timesteps=d._fixed_t, fixed_dofs=d._fixed_d,
                        cart_targets=rep(d.cart_targets), obstacles=rep(d.obstacles) if per_traj else d.obstacles,
-                       obstacles_per_traj=per_traj, sqp=d.c.sqp, qp=d.c.qp, group_size=n_seeds, group_stop=group_stop)
+                       obstacles_per_traj=per_traj, sqp=d.c.sqp, qp=d.c.qp, group_size=n_seeds, group_stop=group_stop,
+                       sqp_per_traj=None if d.sqp_per_traj is None else [r for r in d.sqp_per_traj for _ in range(n_seeds)])
 
 
 def config3(B=4096, T=50, seed=SEED + 3, n_obstacles=8, via_every=10, lvs=0.05, evaluator=COLL_LVS_CONTINUOUS):
@@ -380,5 +381,23 @@ def config4(B=256, T=40, seed=SEED + 4, n_obstacles=8, trust_box_size=None, trus
 
 # the trust-region sweep of configs[4] (SURVEY.md section 8d)
 CONFIG4_SWEEP = [(tb, sh, ex) for tb in (0.01, 0.05, 0.1, 0.5) for sh in (0.1, 0.5) for ex in (1.2, 1.5, 2.0)]
+
+
+def sweep(desc, param_sets):
+    """A parameter sweep as one batch: the description tiled once per parameter set (capi.SqpParams), trajectories
+    [k*B, (k+1)*B) running under param_sets[k].  Returns the tiled description, whose per-trajectory table holds those
+    rows, and the set index of every trajectory ([len(param_sets) * B]).  Groups stay whole: every tile is the whole
+    batch."""
+    d, K = desc, len(param_sets)
+    if K < 1:
+        raise ValueError("no parameter sets")
+    tile = lambda a: None if a is None else np.concatenate([a] * K, axis=0)  # noqa: E731
+    per_traj = bool(d.c.obstacles_per_traj)
+    rows = [p for p in param_sets for _ in range(d.B)]
+    out = ProblemDesc(d.robot_spec, d.T, d.terms, tile(d.init_traj), fixed_timesteps=d._fixed_t, fixed_dofs=d._fixed_d,
+                      cart_targets=tile(d.cart_targets), obstacles=tile(d.obstacles) if per_traj else d.obstacles,
+                      obstacles_per_traj=per_traj, sqp=d.c.sqp, qp=d.c.qp, group_size=d.c.group_size,
+                      group_stop=d.c.group_stop, sqp_per_traj=rows)
+    return out, np.repeat(np.arange(K, dtype=np.int32), d.B)
 
 CONFIGS = {"cfg0": config0, "cfg1": config1, "cfg2": config2, "cfg3": config3, "cfg4": config4, "variants": config_variants}
