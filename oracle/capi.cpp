@@ -2,6 +2,7 @@
 // tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference leg only.
 #include <chrono>
 #include <cstring>
+#include <limits>
 #include <string>
 
 #include "trajopt.hpp"
@@ -30,6 +31,8 @@ Layout layoutOf(const tb200_problem_desc& d, const TrajProblem& tp) {
     } else if (t.kind == TB200_TERM_CART_VEL) {
       L.n_cart_rows += 6 * (t.last_step - t.first_step + 1);
       has_vel = true;
+    } else if (t.kind == TB200_TERM_AVOID_SINGULARITY) {
+      L.n_cart_rows += t.last_step - t.first_step + 1;
     } else if (t.kind == TB200_TERM_COLLISION) {
       if (t.evaluator_type != TB200_COLL_DISCRETE) {  // one object per step pair, dense over sub-segments
         L.n_coll_cand += (t.last_step - t.first_step) * tb200inl_cast_rows_per_pair(&d);
@@ -48,6 +51,97 @@ Layout layoutOf(const tb200_problem_desc& d, const TrajProblem& tp) {
   L.cart_stride = has_vel ? 2 * D : D;
   L.coll_stride = has_cast ? 2 * D + 3 : D + 3;
   return L;
+}
+void putResults(const TrajProblem& tp, const BasicTrustRegionSQP& opt, int b, tb200_results* out) {
+  const OptResults& r = opt.results();
+  const size_t N = r.x.size(), nc = tp.cost_names.size(), nk = tp.cnt_names.size();
+  if (out->x) std::memcpy(out->x + b * N, r.x.data(), sizeof(double) * N);
+  if (out->status) out->status[b] = r.status;
+  if (out->total_cost) out->total_cost[b] = r.total_cost;
+  if (out->cost_vals)
+    for (size_t i = 0; i < nc; ++i) out->cost_vals[b * nc + i] = r.cost_vals[i];
+  if (out->cnt_viols)
+    for (size_t i = 0; i < nk; ++i) out->cnt_viols[b * nk + i] = r.cnt_viols[i];
+  if (out->n_qp_solves) out->n_qp_solves[b] = r.n_qp_solves;
+  if (out->n_func_evals) out->n_func_evals[b] = r.n_func_evals;
+  if (out->n_admm_iters) out->n_admm_iters[b] = static_cast<int>(tp.prob->model()->totalAdmmIters());
+}
+
+// The iteration log of every trajectory, [B][cap][...] (record k of trajectory b at b * cap + k); any array may be NULL.
+struct oracle_records {
+  int cap;
+  int32_t* n;                // [B] records written (at most cap)
+  double* trace;             // [B][cap][14] the TraceEntry columns of the record's QP solve; NaN for record 0
+  double* merit_coeffs;      // [B][cap][n_cnts]
+  double* model_cost_vals;   // [B][cap][n_costs]
+  double* model_cnt_viols;   // [B][cap][n_cnts]
+  double* cost_vals;         // [B][cap][n_costs]
+  double* cnt_viols;         // [B][cap][n_cnts]
+  double* x;                 // [B][cap][T * D]
+};
+// one TraceEntry as 14 doubles
+void traceRow(const TraceEntry& te, double* o) {
+  o[0] = te.merit_round; o[1] = te.iter; o[2] = te.trust; o[3] = te.old_merit; o[4] = te.model_merit;
+  o[5] = te.new_merit; o[6] = te.qp_status; o[7] = te.admm_iters; o[8] = te.action;
+  o[9] = te.pri; o[10] = te.dua; o[11] = te.rho; o[12] = te.polish; o[13] = te.warm;
+}
+void putRecords(const BasicTrustRegionSQP& opt, int b, const oracle_records& rec) {
+  auto put = [](double* dst, size_t at, const Vec& v) {
+    if (dst) std::memcpy(dst + at * v.size(), v.data(), sizeof(double) * v.size());
+  };
+  const size_t n = std::min(opt.records.size(), static_cast<size_t>(rec.cap));
+  if (rec.n) rec.n[b] = static_cast<int32_t>(n);
+  for (size_t k = 0; k < n; ++k) {
+    const size_t at = static_cast<size_t>(b) * rec.cap + k;
+    if (rec.trace) {
+      double* o = rec.trace + at * 14;
+      if (k == 0)
+        std::fill(o, o + 14, std::numeric_limits<double>::quiet_NaN());
+      else
+        traceRow(opt.trace[k - 1], o);
+    }
+    const IterRecord& r = opt.records[k];
+    put(rec.merit_coeffs, at, r.merit_coeffs);
+    put(rec.model_cost_vals, at, r.model_cost_vals);
+    put(rec.model_cnt_viols, at, r.model_cnt_viols);
+    put(rec.cost_vals, at, r.cost_vals);
+    put(rec.cnt_viols, at, r.cnt_viols);
+    put(rec.x, at, r.x);
+  }
+}
+
+// BasicTrustRegionSQP::optimize() for trajectories [b0, b1) of the batch, OpenMP over trajectories: setup(opt, b)
+// configures a trajectory's driver, collect(opt, b) copies out what the entry point returns beyond the results.
+template <class Setup, class Collect>
+int solveBatch(const tb200_problem_desc* desc, int b0, int b1, int n_threads, tb200_results* out, double* seconds,
+               Setup setup, Collect collect) {
+  int err = 0;
+  const int cast_cap = tb200inl_cast_rows_per_pair(desc);
+  const auto t0 = std::chrono::steady_clock::now();
+#ifdef _OPENMP
+  if (n_threads > 0) omp_set_num_threads(n_threads);
+#endif
+#pragma omp parallel for schedule(dynamic)
+  for (int b = b0; b < b1; ++b) {
+    try {
+      TrajProblem tp = buildProblem(*desc, b, cast_cap);
+      BasicTrustRegionSQP opt(tp.prob);
+      opt.params() = sqpParamsFrom(desc->sqp);
+      setup(opt, b);
+      opt.initialize(tp.init);
+      opt.optimize();
+      putResults(tp, opt, b, out);
+      collect(opt, b);
+    } catch (const std::exception& e) {
+#pragma omp critical
+      {
+        g_err = e.what();
+        err = 1;
+      }
+    }
+  }
+  if (seconds) *seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  return err;
 }
 }  // namespace
 
@@ -73,59 +167,38 @@ int oracle_layout(const tb200_problem_desc* desc, tb200_layout* out) {
   }
 }
 
-// BasicTrustRegionSQP::optimize() for trajectories [b0, b1) of the batch, OpenMP over trajectories.
+// BasicTrustRegionSQP::optimize() for trajectories [b0, b1) of the batch, OpenMP over trajectories; desc->sqp.max_time
+// is not read.  seconds: NULL or the wall time of the whole call.
 // trace_*: optional decision trace of trajectory `trace_b` (max trace_cap entries of 14 doubles).
 int oracle_solve_batch(const tb200_problem_desc* desc, int b0, int b1, int n_threads, tb200_results* out,
                        double* seconds, int trace_b, double* trace_out, int trace_cap, int* trace_len) {
-  const int T = desc->n_steps, D = desc->robot.n_dof;
-  int err = 0;
-  const int cast_cap = tb200inl_cast_rows_per_pair(desc);
-  const auto t0 = std::chrono::steady_clock::now();
-#ifdef _OPENMP
-  if (n_threads > 0) omp_set_num_threads(n_threads);
-#endif
-#pragma omp parallel for schedule(dynamic)
-  for (int b = b0; b < b1; ++b) {
-    try {
-      TrajProblem tp = buildProblem(*desc, b, cast_cap);
-      BasicTrustRegionSQP opt(tp.prob);
-      opt.params() = sqpParamsFrom(desc->sqp);
-      opt.initialize(tp.init);
-      opt.optimize();
-      const OptResults& r = opt.results();
-      const size_t nc = tp.cost_names.size(), nk = tp.cnt_names.size();
-      if (out->x) std::memcpy(out->x + static_cast<size_t>(b) * T * D, r.x.data(), sizeof(double) * T * D);
-      if (out->status) out->status[b] = r.status;
-      if (out->total_cost) out->total_cost[b] = r.total_cost;
-      if (out->cost_vals)
-        for (size_t i = 0; i < nc; ++i) out->cost_vals[b * nc + i] = r.cost_vals[i];
-      if (out->cnt_viols)
-        for (size_t i = 0; i < nk; ++i) out->cnt_viols[b * nk + i] = r.cnt_viols[i];
-      if (out->n_qp_solves) out->n_qp_solves[b] = r.n_qp_solves;
-      if (out->n_func_evals) out->n_func_evals[b] = r.n_func_evals;
-      if (out->n_admm_iters) out->n_admm_iters[b] = static_cast<int>(tp.prob->model()->totalAdmmIters());
-      if (b == trace_b && trace_out) {
-        int n = 0;
-        for (const TraceEntry& te : opt.trace) {
-          if (n >= trace_cap) break;
-          double* o = trace_out + n * 14;
-          o[0] = te.merit_round; o[1] = te.iter; o[2] = te.trust; o[3] = te.old_merit; o[4] = te.model_merit;
-          o[5] = te.new_merit; o[6] = te.qp_status; o[7] = te.admm_iters; o[8] = te.action;
-          o[9] = te.pri; o[10] = te.dua; o[11] = te.rho; o[12] = te.polish; o[13] = te.warm;
-          ++n;
-        }
-        if (trace_len) *trace_len = n;
-      }
-    } catch (const std::exception& e) {
-#pragma omp critical
-      {
-        g_err = e.what();
-        err = 1;
-      }
-    }
-  }
-  if (seconds) *seconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-  return err;
+  return solveBatch(desc, b0, b1, n_threads, out, seconds, [](BasicTrustRegionSQP&, int) {},
+                    [&](const BasicTrustRegionSQP& opt, int b) {
+                      if (b != trace_b || !trace_out) return;
+                      const int n = std::min(static_cast<int>(opt.trace.size()), trace_cap);
+                      for (int k = 0; k < n; ++k) traceRow(opt.trace[k], trace_out + k * 14);
+                      if (trace_len) *trace_len = n;
+                    });
+}
+
+// oracle_solve_batch with a stop rule and the iteration log.
+// stop_rule: 0 none (desc->sqp.max_time is not read), 1 a wall clock per trajectory against desc->sqp.max_time,
+// 2 the QP budget qp_budget[b] ([B]).  ended: [B] or NULL, 1 where the stop rule ended the trajectory.
+// records: NULL, or the iteration log of every trajectory.
+int oracle_solve_batch_ext(const tb200_problem_desc* desc, int b0, int b1, int n_threads, int stop_rule,
+                           const int32_t* qp_budget, tb200_results* out, int32_t* ended, const oracle_records* records,
+                           double* seconds) {
+  return solveBatch(
+      desc, b0, b1, n_threads, out, seconds,
+      [&](BasicTrustRegionSQP& opt, int b) {
+        opt.setStopRule(static_cast<BasicTrustRegionSQP::StopRule>(stop_rule), desc->sqp.max_time,
+                        qp_budget ? qp_budget[b] : 0);
+        opt.record = records != nullptr;
+      },
+      [&](const BasicTrustRegionSQP& opt, int b) {
+        if (ended) ended[b] = opt.ended ? 1 : 0;
+        if (records) putRecords(opt, b, *records);
+      });
 }
 
 // costs[i]->convex/value and cnts[i]->convex/violation at x for trajectories [b0,b1), written in the
@@ -185,39 +258,18 @@ int oracle_qp_solve_batch(const tb200_problem_desc* desc, int b0, int b1, const 
     for (int b = b0; b < b1; ++b) {
       TrajProblem tp = buildProblem(*desc, b, cast_cap);
       Model* model = tp.prob->model();
-      const auto& costs = tp.prob->getCosts();
-      const auto cnts = tp.prob->getConstraints();
+      const size_t nc = tp.cost_names.size(), nk = tp.cnt_names.size();
       Vec xv(x + static_cast<size_t>(b) * N, x + static_cast<size_t>(b + 1) * N);
-      std::vector<std::shared_ptr<ConvexObjective>> cm, ccm;
-      std::vector<std::shared_ptr<ConvexConstraints>> km;
-      for (auto& c : costs) cm.push_back(c->convex(xv, model));
-      for (auto& c : cnts) km.push_back(c->convex(xv, model));
-      for (size_t c = 0; c < km.size(); ++c) {
-        auto obj = std::make_shared<ConvexObjective>(model);
-        const double mu = merit_coeffs[b * cnts.size() + c];
-        for (const AffExpr& a : km[c]->eqs) obj->addAbs(a, mu);
-        for (const AffExpr& a : km[c]->ineqs) obj->addHinge(a, mu);
-        ccm.push_back(obj);
-      }
-      for (auto& c : cm) c->addConstraintsToModel();
-      for (auto& c : ccm) c->addConstraintsToModel();
-      QuadExpr obj;
-      for (auto& c : cm) exprInc(obj, c->quad);
-      for (auto& c : ccm) exprInc(obj, c->quad);
-      model->setObjective(obj);
-      for (int i = 0; i < N; ++i) {
-        const double lb = tp.prob->lower()[i], ub = tp.prob->upper()[i];
-        const double xi = std::min(std::max(xv[i], lb), ub);
-        model->setVarBounds(i, std::max(xi - trust[b], lb), std::min(xi + trust[b], ub));
-      }
+      const ConvexModels cm = convexifyProblem(*tp.prob, xv, merit_coeffs + b * nk);
+      setTrustBoxConstraints(*tp.prob, xv, trust[b]);
       const CvxStatus st = model->optimize();
       const Vec& sol = model->solution();
+      Vec mc, mk;
+      cm.values(sol.data(), mc, mk);
       if (new_x) std::memcpy(new_x + static_cast<size_t>(b) * N, sol.data(), sizeof(double) * N);
       if (qp_status) qp_status[b] = st;
-      if (model_cost_vals)
-        for (size_t i = 0; i < cm.size(); ++i) model_cost_vals[b * cm.size() + i] = cm[i]->value(sol.data());
-      if (model_cnt_viols)
-        for (size_t i = 0; i < km.size(); ++i) model_cnt_viols[b * km.size() + i] = km[i]->violation(sol.data());
+      if (model_cost_vals) std::copy(mc.begin(), mc.end(), model_cost_vals + b * nc);
+      if (model_cnt_viols) std::copy(mk.begin(), mk.end(), model_cnt_viols + b * nk);
       if (admm_iters) admm_iters[b] = model->lastResult().iters;
       if (polish) polish[b] = model->lastResult().polish;
       if (kkt) {
@@ -254,6 +306,48 @@ int oracle_jacobian(const tb200_robot* robot, const double* q, int link, const d
   for (int i = 0; i < 6; ++i) std::memcpy(J + i * r.n_dof, Jv[i].data(), sizeof(double) * r.n_dof);
   return 0;
 }
+// avoid_singularity probes: sigma, u[6], v[D] of a 6 x D matrix (row-major); the Jacobian, sigma, err and the unscaled
+// gradient of one waypoint (any output may be NULL)
+int oracle_sing_svd_min(const double* J, int D, double* sigma, double* u, double* v) {
+  sing::jacobiSvdMin(J, D, *sigma, u, v);
+  return 0;
+}
+int oracle_sing_err_grad(const tb200_robot* robot, const double* q, int link, double lambda, double* J, double* sigma,
+                         double* err, double* grad) {
+  try {
+    Robot r(*robot);
+    std::vector<double> Jv;
+    sing::jacobianAt(r, q, link, Jv);
+    if (J) std::memcpy(J, Jv.data(), sizeof(double) * Jv.size());
+    sing::errGrad(r, q, link, lambda, err, grad, sigma);
+    return 0;
+  } catch (const std::exception& e) {
+    g_err = e.what();
+    return 1;
+  }
+}
+
+// (term, step) of every object in OptProb order (the costs, then the EQ and the INEQ constraints), as
+// tb200_problem_objects lists them; term and step: [n_costs + n_cnts]
+int oracle_objects(const tb200_problem_desc* desc, int32_t* term, int32_t* step) {
+  try {
+    TrajProblem tp = buildProblem(*desc, 0);
+    int n = 0;
+    for (const auto& c : tp.prob->getCosts()) {
+      term[n] = c->term;
+      step[n++] = c->step;
+    }
+    for (const auto& c : tp.prob->getConstraints()) {
+      term[n] = c->term;
+      step[n++] = c->step;
+    }
+    return 0;
+  } catch (const std::exception& e) {
+    g_err = e.what();
+    return 1;
+  }
+}
+
 void oracle_transform_error(const double* t1 /*xyz+wxyz*/, const double* t2, double* err6) {
   calcTransformError(poseFromXyzWxyz(t1, t1 + 3), poseFromXyzWxyz(t2, t2 + 3), err6);
 }

@@ -5,6 +5,7 @@
 
 #include <algorithm>
 #include <cassert>
+#include <chrono>
 #include <cstdio>
 #include <cstdlib>
 #include <numeric>
@@ -1202,14 +1203,42 @@ void trustBox(double x, double lb, double ub, double trust, double& lo, double& 
   lo = std::max(xi - trust, lb);
   hi = std::min(xi + trust, ub);
 }
-void BasicTrustRegionSQP::setTrustBoxConstraints(const Vec& x) {
-  const Vec& lb = prob_->lower();
-  const Vec& ub = prob_->upper();
+void setTrustBoxConstraints(OptProb& prob, const Vec& x, double trust) {
+  const Vec& lb = prob.lower();
+  const Vec& ub = prob.upper();
   for (size_t i = 0; i < x.size(); ++i) {
     double lo, hi;
-    trustBox(x[i], lb[i], ub[i], param_.trust_box_size, lo, hi);
-    prob_->model()->setVarBounds(static_cast<int>(i), lo, hi);
+    trustBox(x[i], lb[i], ub[i], trust, lo, hi);
+    prob.model()->setVarBounds(static_cast<int>(i), lo, hi);
   }
+}
+
+ConvexModels convexifyProblem(OptProb& prob, const Vec& x, const double* merit_coeffs) {
+  Model* model = prob.model();
+  ConvexModels out;
+  model->truncateToPermanent();
+  std::vector<std::shared_ptr<ConvexObjective>> cnt_cost_models;
+  for (auto& c : prob.getCosts()) out.costs.push_back(c->convex(x, model));
+  for (auto& c : prob.getConstraints()) out.cnts.push_back(c->convex(x, model));
+  for (size_t c = 0; c < out.cnts.size(); ++c) {
+    auto obj = std::make_shared<ConvexObjective>(model);
+    for (const AffExpr& a : out.cnts[c]->eqs) obj->addAbs(a, merit_coeffs[c]);
+    for (const AffExpr& a : out.cnts[c]->ineqs) obj->addHinge(a, merit_coeffs[c]);
+    cnt_cost_models.push_back(obj);
+  }
+  for (auto& c : out.costs) c->addConstraintsToModel();
+  for (auto& c : cnt_cost_models) c->addConstraintsToModel();
+  QuadExpr objective;
+  for (auto& c : out.costs) exprInc(objective, c->quad);
+  for (auto& c : cnt_cost_models) exprInc(objective, c->quad);
+  model->setObjective(objective);
+  return out;
+}
+void ConvexModels::values(const double* x, Vec& cost_vals, Vec& cnt_viols) const {
+  cost_vals.resize(costs.size());
+  cnt_viols.resize(cnts.size());
+  for (size_t i = 0; i < costs.size(); ++i) cost_vals[i] = costs[i]->value(x);
+  for (size_t i = 0; i < cnts.size(); ++i) cnt_viols[i] = cnts[i]->violation(x);
 }
 
 static double vecSum(const Vec& v) {
@@ -1234,6 +1263,10 @@ OptStatus BasicTrustRegionSQP::optimize() {
   results_.x = prob_->getClosestFeasiblePoint(results_.x);
   OptStatus retval = OPT_INVALID;
   trace.clear();
+  records.clear();
+  ended = false;
+  const auto start = stop_ == STOP_WALL_CLOCK ? std::chrono::steady_clock::now() : std::chrono::steady_clock::time_point();
+  const double nan = std::numeric_limits<double>::quiet_NaN();
 
   auto evalCosts = [&](const Vec& x) {
     Vec out(costs.size());
@@ -1245,6 +1278,11 @@ OptStatus BasicTrustRegionSQP::optimize() {
     for (size_t i = 0; i < constraints.size(); ++i) out[i] = constraints[i]->violation(x);
     return out;
   };
+  auto feasible = [&] { return results_.cnt_viols.empty() || vecMax(results_.cnt_viols) < param_.cnt_tolerance; };
+  auto failedRecord = [&] {
+    return IterRecord{merit_error_coeffs, Vec(costs.size(), nan), Vec(constraints.size(), nan),
+                      Vec(costs.size(), nan), Vec(constraints.size(), nan), Vec(results_.x.size(), nan)};
+  };
 
   for (int merit_increases = 0; merit_increases < param_.max_merit_coeff_increases; ++merit_increases) {
     for (int iter = 1;; ++iter) {
@@ -1252,34 +1290,31 @@ OptStatus BasicTrustRegionSQP::optimize() {
         results_.cnt_viols = evalViols(results_.x);
         results_.cost_vals = evalCosts(results_.x);
         ++results_.n_func_evals;
+        if (record)
+          records.push_back({merit_error_coeffs, Vec(costs.size(), nan), Vec(constraints.size(), nan),
+                             results_.cost_vals, results_.cnt_viols, results_.x});
       }
-      // convexify (optimizers.cpp:781-799); the previous iteration's aux vars / rows are dropped
-      model->truncateToPermanent();
-      std::vector<std::shared_ptr<ConvexObjective>> cost_models, cnt_cost_models;
-      std::vector<std::shared_ptr<ConvexConstraints>> cnt_models;
-      for (auto& c : costs) cost_models.push_back(c->convex(results_.x, model));
-      for (auto& c : constraints) cnt_models.push_back(c->convex(results_.x, model));
-      for (size_t c = 0; c < cnt_models.size(); ++c) {  // cntsToCosts, optimizers.cpp:59-81
-        auto obj = std::make_shared<ConvexObjective>(model);
-        for (const AffExpr& a : cnt_models[c]->eqs) obj->addAbs(a, merit_error_coeffs[c]);
-        for (const AffExpr& a : cnt_models[c]->ineqs) obj->addHinge(a, merit_error_coeffs[c]);
-        cnt_cost_models.push_back(obj);
+      if (stop_ != STOP_NONE) {  // the iteration top: the stop rule, never on a retry below
+        const bool over = stop_ == STOP_QP_BUDGET
+                              ? results_.n_qp_solves >= qp_budget_
+                              : std::chrono::duration<double>(std::chrono::steady_clock::now() - start).count() > max_time_;
+        if (over) {
+          ended = true;
+          retval = feasible() ? OPT_CONVERGED : OPT_TIME_LIMIT;
+          goto cleanup;
+        }
       }
-      for (auto& c : cost_models) c->addConstraintsToModel();
-      for (auto& c : cnt_cost_models) c->addConstraintsToModel();
-      QuadExpr objective;
-      for (auto& c : cost_models) exprInc(objective, c->quad);
-      for (auto& c : cnt_cost_models) exprInc(objective, c->quad);
-      model->setObjective(objective);
+      const ConvexModels cm = convexifyProblem(*prob_, results_.x, merit_error_coeffs.data());
 
       int qp_solver_failures = 0;
       while (param_.trust_box_size >= param_.min_trust_box_size) {
-        setTrustBoxConstraints(results_.x);
+        setTrustBoxConstraints(*prob_, results_.x, param_.trust_box_size);
         const CvxStatus status = model->optimize();
         ++results_.n_qp_solves;
         if (status != CVX_SOLVED) {
           trace.push_back({merit_increases, iter, param_.trust_box_size, 0, 0, 0, model->lastResult().status,
                            model->lastResult().iters, 3});
+          if (record) records.push_back(failedRecord());
           if (qp_solver_failures < (param_.max_qp_solver_failures - 1)) {
             param_.trust_box_size *= param_.trust_shrink_ratio;
             qp_solver_failures++;
@@ -1295,9 +1330,8 @@ OptStatus BasicTrustRegionSQP::optimize() {
         }
         // BasicTrustRegionSQPResults::update, optimizers.cpp:380-426
         const Vec& mv = model->solution();
-        Vec model_cost_vals(cost_models.size()), model_cnt_viols(cnt_models.size());
-        for (size_t i = 0; i < cost_models.size(); ++i) model_cost_vals[i] = cost_models[i]->value(mv.data());
-        for (size_t i = 0; i < cnt_models.size(); ++i) model_cnt_viols[i] = cnt_models[i]->violation(mv.data());
+        Vec model_cost_vals, model_cnt_viols;
+        cm.values(mv.data(), model_cost_vals, model_cnt_viols);
         Vec new_x(mv.begin(), mv.begin() + static_cast<long>(results_.x.size()));
         const Vec new_cost_vals = evalCosts(new_x);
         const Vec new_cnt_viols = evalViols(new_x);
@@ -1315,6 +1349,8 @@ OptStatus BasicTrustRegionSQP::optimize() {
         te.rho = model->lastResult().rho;
         te.polish = model->lastResult().polish;
         te.warm = model->lastResult().warm;
+        if (record)
+          records.push_back({merit_error_coeffs, model_cost_vals, model_cnt_viols, new_cost_vals, new_cnt_viols, new_x});
 
         if (approx_merit_improve < param_.min_approx_improve) {
           te.action = 2;
@@ -1346,12 +1382,12 @@ OptStatus BasicTrustRegionSQP::optimize() {
         goto penaltyadjustment;
       } else if (iter >= param_.max_iter) {
         retval = OPT_SCO_ITERATION_LIMIT;
-        if (results_.cnt_viols.empty() || vecMax(results_.cnt_viols) < param_.cnt_tolerance) retval = OPT_CONVERGED;
+        if (feasible()) retval = OPT_CONVERGED;
         goto cleanup;
       }
     }
   penaltyadjustment:
-    if (results_.cnt_viols.empty() || vecMax(results_.cnt_viols) < param_.cnt_tolerance) {
+    if (feasible()) {
       goto cleanup;
     } else {
       if (param_.inflate_constraints_individually) {

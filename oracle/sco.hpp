@@ -211,6 +211,7 @@ public:
   virtual double value(const Vec& x) = 0;
   virtual std::shared_ptr<ConvexObjective> convex(const Vec& x, Model* model) = 0;
   std::string name;
+  int term = -1, step = -1;  // the description term and step the object was made for
 };
 class Constraint {
 public:
@@ -221,6 +222,7 @@ public:
   Vec violations(const Vec& x);       // modeling.cpp:150-167
   double violation(const Vec& x);     // modeling.cpp:169
   std::string name;
+  int term = -1, step = -1;  // the description term and step the object was made for
 };
 
 class OptProb {  // modeling.cpp:170-271
@@ -334,22 +336,57 @@ struct TraceEntry {
   int polish = 0, warm = 0;
 };
 
+// One entry of the iteration log.  Record 0 is the state after the first evaluation (the clamped start, its exact
+// values, the initial merit coefficients); record k >= 1 is the QP solve of trace[k - 1]: the merit coefficients in
+// force, the model value of every object at the QP solution, the exact values there and the point.  What a record
+// does not have (record 0's model values; a failed QP's model values, exact values and point) is NaN.
+struct IterRecord {
+  Vec merit_coeffs, model_cost_vals, model_cnt_viols, cost_vals, cnt_viols, x;
+};
+
 void trustBox(double x, double lb, double ub, double trust, double& lo, double& hi);  // optimizers.cpp:163-168
+// every variable's trust box around x (setTrustBoxConstraints, optimizers.cpp:151-170)
+void setTrustBoxConstraints(OptProb& prob, const Vec& x, double trust);
+
+// The QP of one SQP iteration at x (optimizers.cpp:781-799): the previous iteration's aux vars / rows dropped, every
+// cost and constraint convexified, the constraints made costs with their merit coefficients (cntsToCosts,
+// optimizers.cpp:59-81), their rows added to the model and the summed objective set.  The trust box is not set.
+struct ConvexModels {
+  std::vector<std::shared_ptr<ConvexObjective>> costs;
+  std::vector<std::shared_ptr<ConvexConstraints>> cnts;
+  // the model's values at x: the costs' values and the constraints' violations
+  void values(const double* x, Vec& cost_vals, Vec& cnt_viols) const;
+};
+ConvexModels convexifyProblem(OptProb& prob, const Vec& x, const double* merit_coeffs);
 
 class BasicTrustRegionSQP {
 public:
+  // When the run stops early (optimizers.cpp:738-753): never, on a steady_clock started in optimize() past max_time,
+  // or at the first iteration top with n_qp_solves >= qp_budget.
+  enum StopRule { STOP_NONE, STOP_WALL_CLOCK, STOP_QP_BUDGET };
+
   explicit BasicTrustRegionSQP(std::shared_ptr<OptProb> prob) : prob_(std::move(prob)) {}
   SQPParams& params() { return param_; }
   void initialize(const Vec& x) { results_ = OptResults(); results_.x = x; }
+  void setStopRule(StopRule rule, double max_time, int qp_budget) {
+    stop_ = rule;
+    max_time_ = max_time;
+    qp_budget_ = qp_budget;
+  }
   OptStatus optimize();  // optimizers.cpp:699-991
   const OptResults& results() const { return results_; }
   std::vector<TraceEntry> trace;
+  bool ended = false;                // the stop rule ended the run
+  bool record = false;               // fill `records`
+  std::vector<IterRecord> records;
 
 private:
-  void setTrustBoxConstraints(const Vec& x);  // optimizers.cpp:151-170
   std::shared_ptr<OptProb> prob_;
   SQPParams param_;
   OptResults results_;
+  StopRule stop_ = STOP_NONE;
+  double max_time_ = 0;
+  int qp_budget_ = 0;
 };
 
 }  // namespace oracle

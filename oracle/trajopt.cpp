@@ -654,6 +654,105 @@ private:
 };
 }  // namespace
 
+// ============================================================================ avoid_singularity
+// AvoidSingularityTermInfo (kinematic_terms.cpp:586-642): err = 1/(s + lambda) - 1/(0.1 + lambda), s the smallest
+// singular value of the 6 x D geometric Jacobian of the link's origin, by a one-sided Jacobi SVD (the rotation order
+// and stopping rule of the device's); the gradient is the reference's forward difference
+// g_j = u' ((J(q + eps e_j) - J(q)) / eps) v, eps = 1e-6, times -1 / (s + lambda)^2.
+namespace sing {
+namespace {
+constexpr double kEps = 1e-6, kUlp = 2.220446049250313e-16;  // rotations stop at |a_p.a_q| <= M kUlp |a_p||a_q|
+constexpr int kSweeps = 32;
+}  // namespace
+
+void jacobiSvdMin(const double* J, int D, double& sigma, double* u, double* v) {
+  const int NC = D < 6 ? D : 6, M = D < 6 ? 6 : D;
+  std::vector<double> A(static_cast<size_t>(M) * NC), V(static_cast<size_t>(NC) * NC, 0.0);  // row-major
+  for (int i = 0; i < M; ++i)
+    for (int k = 0; k < NC; ++k) A[i * NC + k] = D < 6 ? J[i * D + k] : J[k * D + i];
+  for (int k = 0; k < NC; ++k) V[k * NC + k] = 1.0;
+  auto dot = [&](int p, int q) {
+    double s = 0.0;
+    for (int i = 0; i < M; ++i) s += A[i * NC + p] * A[i * NC + q];
+    return s;
+  };
+  for (int sweep = 0; sweep < kSweeps; ++sweep) {
+    bool rotated = false;
+    for (int p = 0; p < NC - 1; ++p)
+      for (int q = p + 1; q < NC; ++q) {
+        const double al = dot(p, p), be = dot(q, q), ga = dot(p, q);
+        if (!(std::fabs(ga) > M * kUlp * std::sqrt(al * be))) continue;
+        const double zeta = (be - al) / (2.0 * ga);
+        const double t = (zeta >= 0.0 ? 1.0 : -1.0) / (std::fabs(zeta) + std::sqrt(1.0 + zeta * zeta));
+        const double c = 1.0 / std::sqrt(1.0 + t * t), s = c * t;
+        for (int i = 0; i < M; ++i) {
+          const double ap = A[i * NC + p], aq = A[i * NC + q];
+          A[i * NC + p] = c * ap - s * aq;
+          A[i * NC + q] = s * ap + c * aq;
+        }
+        for (int i = 0; i < NC; ++i) {
+          const double vp = V[i * NC + p], vq = V[i * NC + q];
+          V[i * NC + p] = c * vp - s * vq;
+          V[i * NC + q] = s * vp + c * vq;
+        }
+        rotated = true;
+      }
+    if (!rotated) break;
+  }
+  int kmin = 0;
+  sigma = 0.0;
+  for (int k = 0; k < NC; ++k) {
+    const double sk = std::sqrt(dot(k, k));
+    if (k == 0 || sk < sigma) {
+      sigma = sk;
+      kmin = k;
+    }
+  }
+  double* w = D < 6 ? u : v;   // W_k / sigma
+  double* vk = D < 6 ? v : u;  // V_k
+  for (int i = 0; i < M; ++i) w[i] = sigma > 0.0 ? A[i * NC + kmin] / sigma : 0.0;
+  for (int i = 0; i < NC; ++i) vk[i] = V[i * NC + kmin];
+}
+
+void jacobianAt(const Robot& robot, const double* q, int link, std::vector<double>& J) {
+  std::vector<Pose> fr;
+  robot.fk(q, fr);
+  std::vector<Vec> Jv;
+  robot.jacobian(fr, link, fr[link].p, Jv);
+  const int D = robot.n_dof;
+  J.assign(6 * D, 0.0);
+  for (int i = 0; i < 6; ++i)
+    for (int j = 0; j < D; ++j) J[i * D + j] = Jv[i][j];
+}
+
+void errGrad(const Robot& robot, const double* q, int link, double lambda, double* err, double* grad, double* sigma_out) {
+  const int D = robot.n_dof;
+  std::vector<double> J0, Jk;
+  jacobianAt(robot, q, link, J0);
+  double sigma, u[6], v[16];
+  jacobiSvdMin(J0.data(), D, sigma, u, v);
+  if (err) *err = 1.0 / (sigma + lambda) - 1.0 / (0.1 + lambda);
+  if (sigma_out) *sigma_out = sigma;
+  if (!grad) return;
+  std::vector<double> qk(q, q + D), dJ(6 * D);
+  for (int j = 0; j < D; ++j) {
+    qk[j] = q[j] + kEps;
+    jacobianAt(robot, qk.data(), link, Jk);
+    qk[j] = q[j];
+    for (int e = 0; e < 6 * D; ++e) dJ[e] = (Jk[e] - J0[e]) / kEps;  // difference matrix, then the division
+    double g = 0.0;
+    for (int c = 0; c < D; ++c) {  // (u' dJ) v
+      double s = 0.0;
+      for (int i = 0; i < 6; ++i) s += u[i] * dJ[i * D + c];
+      g += s * v[c];
+    }
+    grad[j] = g;
+  }
+  const double scale = -1.0 / ((sigma + lambda) * (sigma + lambda));
+  for (int j = 0; j < D; ++j) grad[j] *= scale;
+}
+}  // namespace sing
+
 // ============================================================================ problem assembly
 SQPParams sqpParamsFrom(const tb200_sqp_params& p) {
   SQPParams s;
@@ -744,6 +843,18 @@ TrajProblem buildProblem(const tb200_problem_desc& desc, int b, int cast_cap) {
     const tb200_term& tm = desc.terms[k];
     const bool is_cost = tm.role == TB200_ROLE_COST;
     const std::string nm = "term" + std::to_string(k);
+    auto addCost = [&](std::shared_ptr<Cost> c, const std::string& name, int step) {
+      c->name = name;
+      c->term = k;
+      c->step = step;
+      tp.prob->addCost(c);
+    };
+    auto addCnt = [&](std::shared_ptr<Constraint> c, const std::string& name, int step) {
+      c->name = name;
+      c->term = k;
+      c->step = step;
+      tp.prob->addConstraint(c);
+    };
     switch (tm.kind) {
       case TB200_TERM_JOINT_POS:
       case TB200_TERM_JOINT_VEL:
@@ -763,14 +874,12 @@ TrajProblem buildProblem(const tb200_problem_desc& desc, int b, int cast_cap) {
           std::shared_ptr<Cost> c;
           if (zero_tol) c = std::make_shared<JointEqCost>(s);
           else c = std::make_shared<JointIneqCost>(s);
-          c->name = nm;
-          tp.prob->addCost(c);
+          addCost(c, nm, tm.first_step);
         } else {
           std::shared_ptr<Constraint> c;
           if (zero_tol) c = std::make_shared<JointEqConstraint>(s);
           else c = std::make_shared<JointIneqConstraint>(s);
-          c->name = nm;
-          tp.prob->addConstraint(c);
+          addCnt(c, nm, tm.first_step);
         }
         break;
       }
@@ -827,15 +936,10 @@ TrajProblem buildProblem(const tb200_problem_desc& desc, int b, int cast_cap) {
             jac.push_back(J[r]);
           }
         });
-        if (is_cost) {
-          auto c = std::make_shared<CostFromErrFunc>(f, dfdx, vars, coeff, ABS);
-          c->name = nm;
-          tp.prob->addCost(c);
-        } else {
-          auto c = std::make_shared<ConstraintFromErrFunc>(f, dfdx, vars, coeff, EQ);
-          c->name = nm;
-          tp.prob->addConstraint(c);
-        }
+        if (is_cost)
+          addCost(std::make_shared<CostFromErrFunc>(f, dfdx, vars, coeff, ABS), nm, tm.first_step);
+        else
+          addCnt(std::make_shared<ConstraintFromErrFunc>(f, dfdx, vars, coeff, EQ), nm, tm.first_step);
         break;
       }
       case TB200_TERM_CART_VEL: {
@@ -888,15 +992,10 @@ TrajProblem buildProblem(const tb200_problem_desc& desc, int b, int cast_cap) {
               jac.push_back(J[r]);
             }
           });
-          if (is_cost) {
-            auto c = std::make_shared<CostFromErrFunc>(f, dfdx, vars, Vec(), ABS);
-            c->name = nm + "_" + std::to_string(t);
-            tp.prob->addCost(c);
-          } else {
-            auto c = std::make_shared<ConstraintFromErrFunc>(f, dfdx, vars, Vec(), INEQ);
-            c->name = "CartVel";
-            tp.prob->addConstraint(c);
-          }
+          if (is_cost)
+            addCost(std::make_shared<CostFromErrFunc>(f, dfdx, vars, Vec(), ABS), nm + "_" + std::to_string(t), t);
+          else
+            addCnt(std::make_shared<ConstraintFromErrFunc>(f, dfdx, vars, Vec(), INEQ), "CartVel", t);
         }
         break;
       }
@@ -916,15 +1015,10 @@ TrajProblem buildProblem(const tb200_problem_desc& desc, int b, int cast_cap) {
             CastCollisionEval e{tp.robot, obstacles, t, D, tm.margin, tm.coeff, tm.margin_buffer, lvs, cur_fixed,
                                 !cur_fixed && next_fixed, cast_cap, tm.evaluator_type == TB200_COLL_LVS_DISCRETE};
             tp.coll_hooks.push_back([e](const Vec& x, std::vector<Vec>& rows) { e.denseRows(x, rows); });
-            if (is_cost) {
-              auto c = std::make_shared<CollisionCost>(calcOf(e));
-              c->name = nm + "_" + std::to_string(t);
-              tp.prob->addCost(c);
-            } else {
-              auto c = std::make_shared<CollisionConstraint>(calcOf(e));
-              c->name = nm + "_" + std::to_string(t);
-              tp.prob->addConstraint(c);
-            }
+            if (is_cost)
+              addCost(std::make_shared<CollisionCost>(calcOf(e)), nm + "_" + std::to_string(t), t);
+            else
+              addCnt(std::make_shared<CollisionConstraint>(calcOf(e)), nm + "_" + std::to_string(t), t);
           }
           break;
         }
@@ -935,15 +1029,47 @@ TrajProblem buildProblem(const tb200_problem_desc& desc, int b, int cast_cap) {
           if (fixed) continue;
           CollisionEval e{tp.robot, obstacles, t, D, tm.margin, tm.coeff, tm.margin_buffer};
           tp.coll_hooks.push_back([e](const Vec& x, std::vector<Vec>& rows) { e.denseRows(x, rows); });
-          if (is_cost) {
-            auto c = std::make_shared<CollisionCost>(calcOf(e));
-            c->name = nm + "_" + std::to_string(t);
-            tp.prob->addCost(c);
-          } else {
-            auto c = std::make_shared<CollisionConstraint>(calcOf(e));
-            c->name = nm + "_" + std::to_string(t);
-            tp.prob->addConstraint(c);
-          }
+          if (is_cost)
+            addCost(std::make_shared<CollisionCost>(calcOf(e)), nm + "_" + std::to_string(t), t);
+          else
+            addCnt(std::make_shared<CollisionConstraint>(calcOf(e)), nm + "_" + std::to_string(t), t);
+        }
+        break;
+      }
+      case TB200_TERM_AVOID_SINGULARITY: {
+        // AvoidSingularityTermInfo::hatch (problem_description.cpp:1900-1939): one object per step, ABS cost or INEQ
+        // constraint, and one coefficient-scaled Cartesian row per step
+        if (tm.link < 0 || tm.link >= desc.robot.n_segments) throw std::runtime_error("avoid_singularity link out of range");
+        if (tm.first_step < 0 || tm.last_step >= T || tm.first_step > tm.last_step)
+          throw std::runtime_error("avoid_singularity steps outside the trajectory");
+        auto robot = tp.robot;
+        const int link = tm.link;
+        const double lambda = tm.lambda, coeff = tm.coeffs[0];
+        for (int t = tm.first_step; t <= tm.last_step; ++t) {
+          std::vector<int> vars(D);
+          for (int j = 0; j < D; ++j) vars[j] = t * D + j;
+          VectorFn f = [robot, link, lambda](const Vec& q) {
+            Vec e(1);
+            sing::errGrad(*robot, q.data(), link, lambda, &e[0], nullptr, nullptr);
+            return e;
+          };
+          MatrixFn dfdx = [robot, link, lambda](const Vec& q) {
+            std::vector<Vec> g(1, Vec(q.size()));
+            sing::errGrad(*robot, q.data(), link, lambda, nullptr, g[0].data(), nullptr);
+            return g;
+          };
+          tp.cart_hooks.push_back([=](const Vec& x, Vec& err, std::vector<Vec>& jac) {
+            double e;
+            Vec g(D);
+            sing::errGrad(*robot, x.data() + t * D, link, lambda, &e, g.data(), nullptr);
+            err.push_back(coeff * e);
+            for (double& v : g) v = coeff * v;
+            jac.push_back(g);
+          });
+          if (is_cost)
+            addCost(std::make_shared<CostFromErrFunc>(f, dfdx, vars, Vec{coeff}, ABS), nm + "_" + std::to_string(t), t);
+          else
+            addCnt(std::make_shared<ConstraintFromErrFunc>(f, dfdx, vars, Vec{coeff}, INEQ), nm + "_" + std::to_string(t), t);
         }
         break;
       }

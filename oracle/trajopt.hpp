@@ -59,6 +59,15 @@ struct TrajProblem {
   // dense candidate collision rows [(sphere, obstacle)] = {grad[D], dist0, margin, coeff or 0 if filtered}
   std::vector<std::function<void(const Vec& x, std::vector<Vec>& rows)>> coll_hooks;
 };
+// avoid_singularity: J [6][D] row-major -> its smallest singular value and singular vectors u[6], v[D] (the undefined
+// one of the pair is 0 when sigma is 0); the geometric Jacobian [6][D] of the link's origin at q; err and the
+// unscaled gradient of one waypoint (any output may be NULL)
+namespace sing {
+void jacobiSvdMin(const double* J, int D, double& sigma, double* u, double* v);
+void jacobianAt(const Robot& robot, const double* q, int link, std::vector<double>& J);
+void errGrad(const Robot& robot, const double* q, int link, double lambda, double* err, double* grad, double* sigma_out);
+}  // namespace sing
+
 // One trajectory `b` of the batched description -> the reference's TrajOptProb
 // (ConstructProblem, problem_description.cpp:410-542).
 // cast_cap: rows per step pair of the continuous collision evaluator's fixed-layout output (< 0: compute it,

@@ -3,8 +3,8 @@
 A group is G contiguous trajectories, the seeds of one problem.  With group_stop a seed that ends OPT_CONVERGED by its
 own SQP ends its running siblings at their next SQP iteration top, under the time-limit rule; the best seed of every
 group is selected on the device by the key (status != OPT_CONVERGED, max(cnt_viols) when not converged, total_cost,
-index), NaN read as +inf.  `select_cpu` below restates that key; the CPU model of an early-ended run is
-tests/cpp/time_limit_oracle.cpp with its QP-budget clock.
+index), NaN read as +inf.  `select_cpu` below restates that key; the CPU model of an early-ended run is the oracle's
+SQP driver with its QP-budget stop rule (oracle_lib.solve_batch(..., qp_budget=)).
 CPU: validation before the device, the key on synthetic results, seed_trajectories, sharding on group boundaries, the
 C++ layer's flattening.  GPU (-m gpu): the device against the ungrouped solve, the CPU selection and the CPU model."""
 import ctypes as C
@@ -25,33 +25,6 @@ RESULT_KEYS = ("status", "n_qp_solves", "n_func_evals", "n_admm_iters", "x", "to
 
 
 # ---------------------------------------------------------------------------------------------------------- fixtures
-@pytest.fixture(scope="module")
-def timed(oracle, tmp_path_factory):
-    """tests/cpp/time_limit_oracle.cpp, unchanged: the oracle's SQP driver with the iteration-top check, whose QP-budget
-    clock ("stop at the first iteration top with n_qp_solves >= budget") reproduces an early-ended device run."""
-    out = str(tmp_path_factory.mktemp("ms_tl") / "libtl_oracle.so")
-    lib = os.path.join(ROOT, "oracle", "liboracle.so")
-    cmd = ["g++", "-std=c++17", "-O3", "-march=x86-64-v3", "-fopenmp", "-fPIC", "-DNDEBUG", "-shared",
-           "-I", os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tests", "cpp", "time_limit_oracle.cpp"), lib,
-           "-Wl,-rpath," + os.path.dirname(lib), "-o", out]
-    subprocess.run(cmd, check=True)
-    tl = C.CDLL(out)
-    tl.tl_oracle_last_error.restype = C.c_char_p
-
-    def solve(desc, qp_budget):
-        import oracle_lib
-        L = oracle_lib.layout(desc)
-        buf, res = capi.alloc_results(desc.B, desc.T, desc.D, L.n_costs, L.n_cnts)
-        budget = np.ascontiguousarray(qp_budget, dtype=np.int32)
-        ended = np.zeros(desc.B, np.int32)
-        rc = tl.tl_oracle_solve_batch(C.byref(desc.c), 0, desc.B, budget.ctypes.data_as(_i32_p), C.byref(res),
-                                      ended.ctypes.data_as(_i32_p))
-        assert rc == 0, tl.tl_oracle_last_error()
-        buf["ended"] = ended
-        return buf
-    return solve
-
-
 @pytest.fixture(scope="module")
 def host_bin(tmp_path_factory):
     capi.load_library()  # the CUDA build must exist (no GPU needed to load it)
@@ -348,7 +321,7 @@ def test_device_stop0_is_the_ungrouped_solve_plus_the_selection(runs, name):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", sorted(CASES))
-def test_device_stop1_ends_siblings_of_a_converged_seed(runs, timed, name):
+def test_device_stop1_ends_siblings_of_a_converged_seed(runs, oracle, name):
     d, G, _, ref, got = runs[name]
     ended = got["groups"]["ended_by"]
     own, cut = ended == 0, ended == 2
@@ -375,7 +348,7 @@ def test_device_stop1_ends_siblings_of_a_converged_seed(runs, timed, name):
     # seeds that ended by their own SQP are the stop-0 results, bit for bit)
     ok = ~_unverified(tl, ll, d.c.qp.max_iter) & cut
     assert ok.sum() >= 0.75 * cut.sum()
-    model = timed(d, got["n_qp_solves"])
+    model = oracle.solve_batch(d, qp_budget=got["n_qp_solves"])
     np.testing.assert_array_equal(got["status"][ok], model["status"][ok])
     np.testing.assert_array_equal(got["n_qp_solves"][ok], model["n_qp_solves"][ok])
     np.testing.assert_allclose(got["total_cost"][ok], model["total_cost"][ok], atol=1e-6)

@@ -424,53 +424,16 @@ def test_cpp_callbacks_and_log_results(host_bin, tmp_path):
     assert len(csv) == 1 + n_cb * (d.T + 1) + 1 and csv[-1] == ""
 
 
-# ------------------------------------------------------------------------------ CPU model of the log (sqp_log_oracle.cpp)
-class LogModel:
-    def __init__(self, path):
-        self.lib = C.CDLL(path)
-        self.lib.slo_last_error.restype = C.c_char_p
-
-    def solve(self, desc, cap=512, b0=0, b1=None):
-        import oracle_lib
-        b1 = desc.B if b1 is None else b1
-        L = oracle_lib.layout(desc)
-        B, nc, nk, N = desc.B, L.n_costs, L.n_cnts, desc.T * desc.D
-        buf, res = capi.alloc_results(B, desc.T, desc.D, nc, nk)
-        out = dict(n_records=np.zeros(B, np.int32), trace=np.full((B, cap, 14), np.nan),
-                   mu=np.full((B, cap, nk), np.nan), model_cost_vals=np.full((B, cap, nc), np.nan),
-                   model_cnt_viols=np.full((B, cap, nk), np.nan), new_cost_vals=np.full((B, cap, nc), np.nan),
-                   new_cnt_viols=np.full((B, cap, nk), np.nan), x=np.full((B, cap, N), np.nan))
-        arr = [out[k].ctypes.data_as(_dbl_p) if out[k].size else None for k in
-               ("trace", "mu", "model_cost_vals", "model_cnt_viols", "new_cost_vals", "new_cnt_viols", "x")]
-        rc = self.lib.slo_solve_batch(C.byref(desc.c), b0, b1, cap, C.byref(res),
-                                      out["n_records"].ctypes.data_as(_i32_p), *arr)
-        assert rc == 0, self.lib.slo_last_error()
-        buf["log"] = out
-        return buf
-
-
-@pytest.fixture(scope="module")
-def log_model(oracle, tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("slo") / "libsqp_log_oracle.so")
-    lib = os.path.join(ROOT, "oracle", "liboracle.so")
-    # the oracle's own flags (oracle/Makefile): the same arithmetic as its own driver
-    cmd = ["g++", "-std=c++17", "-O3", "-march=x86-64-v3", "-fopenmp", "-fPIC", "-DNDEBUG", "-shared",
-           "-I", os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tests", "cpp", "sqp_log_oracle.cpp"), lib,
-           "-Wl,-rpath," + os.path.dirname(lib), "-o", out]
-    subprocess.run(cmd, check=True)
-    return LogModel(out)
-
-
 _SMALL = {"cfg1": lambda: problems.config1(B=4, T=12), "cfg2": lambda: problems.config2(B=4, T=12),
           "cfg4": lambda: problems.config4(B=2, T=12)}
 
 
 @pytest.mark.parametrize("name", list(_SMALL))
-def test_log_model_is_the_oracle_driver(oracle, log_model, name):
-    """The CPU model's final results are the oracle's, bit for bit, and its records' 14 trace columns are the oracle's
-    TraceEntry list; record 0 is the clamped start with its exact values."""
+def test_log_model_is_the_oracle_driver(oracle, name):
+    """With records on, the oracle's final results are those with records off, bit for bit, and its records' 14 trace
+    columns are the oracle's TraceEntry list; record 0 is the clamped start with its exact values."""
     d = _SMALL[name]()
-    got = log_model.solve(d)
+    got = oracle.solve_batch(d, records=512)
     ref = oracle.solve_batch(d)
     for k in ("x", "status", "total_cost", "cost_vals", "cnt_viols", "n_qp_solves", "n_func_evals", "n_admm_iters"):
         assert got[k].tobytes() == ref[k].tobytes(), k
@@ -600,14 +563,14 @@ def test_objects_name_their_terms_and_steps(make):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", ["cfg1", "cfg2", "cfg4", "cfg3"])
-def test_log_against_the_cpu_model(log_model, runs, name):
+def test_log_against_the_cpu_model(oracle, runs, name):
     """Every record of every trajectory against the CPU model of the log: the same count, kinds, (round, iter), actions
     and QP outcomes; merit coefficients, per-object model and exact values and the trust box within 1e-8; the points
     within the final-point rule of test_gpu_parity (1e-5).  configs[3]: the loose rule of test_gpu_parity - its long QPs
     may stop on a different ADMM check - so the decisions of a shared prefix only."""
     d, off, on = runs[name]
     L = on["log"]
-    ref = log_model.solve(d)["log"]
+    ref = oracle.solve_batch(d, records=512)["log"]
     for b in range(d.B):
         n = L["n_records"][b]
         if name == "cfg3":

@@ -2,8 +2,8 @@
 
 The limit is checked at the top of every SQP iteration; a trajectory past it ends with its last accepted iterate,
 OPT_CONVERGED when it has no constraints or max(cnt_viols) < cnt_tolerance, else OPT_TIME_LIMIT.  The CPU model of it
-is tests/cpp/time_limit_oracle.cpp (the oracle's SQP driver plus the check), wrapped below; its QP-budget clock
-("stop at the first iteration top with n_qp_solves >= budget") makes a time-limited device run checkable exactly.
+is the oracle's SQP driver with its wall-clock stop rule (oracle_lib.solve_batch(..., wall_clock=True)); its QP-budget
+rule ("stop at the first iteration top with n_qp_solves >= budget") makes a time-limited device run checkable exactly.
 CPU: defaults, both JSON readers, the CPU model at max_time 0 / DBL_MAX.  GPU (-m gpu): the device against it."""
 import ctypes as C
 import json
@@ -21,40 +21,6 @@ CSRC = os.path.join(ROOT, "trajopt_b200", "csrc")
 DBL_MAX = sys.float_info.max
 _dbl_p = C.POINTER(C.c_double)
 _i32_p = C.POINTER(C.c_int32)
-
-
-# ---------------------------------------------------------------------------------------------- CPU model of the limit
-class TimedOracle:
-    def __init__(self, path):
-        self.lib = C.CDLL(path)
-        self.lib.tl_oracle_last_error.restype = C.c_char_p
-
-    def solve(self, desc, qp_budget=None, b0=0, b1=None):
-        """The oracle's SQP with the time limit: desc.c.sqp.max_time on a per-trajectory wall clock, or, with qp_budget
-        ([B] ints), the QP-budget clock.  Returns the result buffers plus "ended" (1: stopped by the limit)."""
-        import oracle_lib
-        b1 = desc.B if b1 is None else b1
-        L = oracle_lib.layout(desc)
-        buf, res = capi.alloc_results(desc.B, desc.T, desc.D, L.n_costs, L.n_cnts)
-        budget = None if qp_budget is None else np.ascontiguousarray(qp_budget, dtype=np.int32)
-        ended = np.zeros(desc.B, np.int32)
-        rc = self.lib.tl_oracle_solve_batch(C.byref(desc.c), b0, b1, None if budget is None else budget.ctypes.data_as(_i32_p),
-                                            C.byref(res), ended.ctypes.data_as(_i32_p))
-        assert rc == 0, self.lib.tl_oracle_last_error()
-        buf["ended"] = ended
-        return buf
-
-
-@pytest.fixture(scope="module")
-def timed(oracle, tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("tl") / "libtl_oracle.so")
-    lib = os.path.join(ROOT, "oracle", "liboracle.so")
-    # the oracle's own flags (oracle/Makefile): the same arithmetic as its untimed driver
-    cmd = ["g++", "-std=c++17", "-O3", "-march=x86-64-v3", "-fopenmp", "-fPIC", "-DNDEBUG", "-shared",
-           "-I", os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tests", "cpp", "time_limit_oracle.cpp"), lib,
-           "-Wl,-rpath," + os.path.dirname(lib), "-o", out]
-    subprocess.run(cmd, check=True)
-    return TimedOracle(out)
 
 
 @pytest.fixture(scope="module")
@@ -138,9 +104,9 @@ def test_cpp_json_reader_maps_max_time(host_bin, tmp_path, max_time, want):
 
 
 @pytest.mark.parametrize("name", sorted(_MAKERS))
-def test_oracle_max_time_zero_stops_after_the_initial_evaluation(oracle, timed, name):
+def test_oracle_max_time_zero_stops_after_the_initial_evaluation(oracle, name):
     d = _with_max_time(_MAKERS[name](), 0.0)
-    r = timed.solve(d)
+    r = oracle.solve_batch(d, wall_clock=True)
     assert (r["n_qp_solves"] == 0).all() and (r["n_func_evals"] == 1).all() and (r["ended"] == 1).all()
     # the closest feasible point of the initial trajectory (modeling.cpp:261-269, including its overwritten lower clip)
     upper = np.asarray(d.robot_spec["upper"], float)
@@ -157,38 +123,38 @@ def test_oracle_max_time_zero_stops_after_the_initial_evaluation(oracle, timed, 
 
 
 @pytest.mark.parametrize("name", ["cfg1", "cfg2", "variants"])
-def test_oracle_without_a_limit_is_the_default_oracle(oracle, timed, name):
+def test_oracle_without_a_limit_is_the_default_oracle(oracle, name):
     d = _MAKERS[name]()
     ref = oracle.solve_batch(d)
     for t in (DBL_MAX, float("nan"), 1e6):
-        r = timed.solve(_with_max_time(d, t))
+        r = oracle.solve_batch(_with_max_time(d, t), wall_clock=True)
         assert (r["ended"] == 0).all()
         for k in ("status", "n_qp_solves", "n_func_evals", "n_admm_iters", "x", "total_cost", "cost_vals", "cnt_viols"):
             np.testing.assert_array_equal(r[k], ref[k], err_msg=k)
 
 
-def test_oracle_negative_max_time_stops_at_the_first_check(timed):
+def test_oracle_negative_max_time_stops_at_the_first_check(oracle):
     d = _with_max_time(_MAKERS["cfg2"](), -1.0)
-    r = timed.solve(d)
+    r = oracle.solve_batch(d, wall_clock=True)
     assert (r["n_qp_solves"] == 0).all() and (r["ended"] == 1).all()
 
 
 @pytest.mark.parametrize("name", ["cfg2", "variants"])
-def test_oracle_qp_budget_zero_is_max_time_zero(timed, name):
+def test_oracle_qp_budget_zero_is_max_time_zero(oracle, name):
     d = _MAKERS[name]()
-    a = timed.solve(d, qp_budget=np.zeros(d.B, np.int32))
-    b = timed.solve(_with_max_time(d, 0.0))
+    a = oracle.solve_batch(d, qp_budget=np.zeros(d.B, np.int32))
+    b = oracle.solve_batch(_with_max_time(d, 0.0), wall_clock=True)
     for k in ("status", "n_qp_solves", "n_func_evals", "x", "total_cost", "cost_vals", "cnt_viols", "ended"):
         np.testing.assert_array_equal(a[k], b[k], err_msg=k)
 
 
-def test_oracle_qp_budget_stops_at_an_iteration_top(oracle, timed):
+def test_oracle_qp_budget_stops_at_an_iteration_top(oracle):
     """A budget of k QPs ends each trajectory at the first iteration top at or after k QPs: the trajectories that need
     fewer are the untimed ones, the others stop after at least k QPs, never more than one SQP iteration later."""
     d = _MAKERS["cfg2"]()
     full = oracle.solve_batch(d)
     k = 3
-    r = timed.solve(d, qp_budget=np.full(d.B, k, np.int32))
+    r = oracle.solve_batch(d, qp_budget=np.full(d.B, k, np.int32))
     done = full["n_qp_solves"] <= k  # (an untimed run that reaches an iteration top always solves one more QP)
     assert (r["ended"][done] == 0).all()
     for key in ("status", "n_qp_solves", "x", "total_cost"):
@@ -221,12 +187,12 @@ def _device_solve(p, trace_cap=0):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", sorted(_MAKERS))
-def test_device_max_time_zero_matches_oracle(timed, name):
+def test_device_max_time_zero_matches_oracle(oracle, name):
     d = _with_max_time(_MAKERS[name](), 0.0)
     p = api.Problem(d)
     got = _device_solve(p)
     p.close()
-    ref = timed.solve(d)
+    ref = oracle.solve_batch(d, wall_clock=True)
     assert (got["ended"] == 1).all()
     for k in ("status", "n_qp_solves", "n_func_evals", "x"):
         np.testing.assert_array_equal(got[k], ref[k], err_msg=k)
@@ -261,7 +227,7 @@ def _unverified(tr, tl, qp_max_iter):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,make", [("cfg2", lambda: problems.config2(B=256, T=30)),
                                        ("cfg3", lambda: problems.config3(B=32, T=30))])
-def test_device_intermediate_budget(timed, name, make):
+def test_device_intermediate_budget(oracle, name, make):
     d = make()
     cap = 600
     p = api.Problem(d)
@@ -293,7 +259,7 @@ def test_device_intermediate_budget(timed, name, make):
     # against the CPU model with the device's QP counts as budgets, where every QP was KKT-verified
     ok = ~_unverified(tl, ll, d.c.qp.max_iter)
     assert ok.mean() >= 0.75
-    ref = timed.solve(d, qp_budget=lim["n_qp_solves"])
+    ref = oracle.solve_batch(d, qp_budget=lim["n_qp_solves"])
     np.testing.assert_array_equal(lim["status"][ok], ref["status"][ok])
     np.testing.assert_array_equal(lim["n_qp_solves"][ok], ref["n_qp_solves"][ok])
     np.testing.assert_allclose(lim["total_cost"][ok], ref["total_cost"][ok], atol=1e-6)
