@@ -314,6 +314,15 @@ private:
 };
 
 // ============================================================================ collision (discrete)
+// unit normal d / |d| from the robot sphere towards the obstacle; coincident centres (|d| = 0) take the fixed
+// scene-frame normal (1, 0, 0) instead of 0/0 (DESIGN.md section 6, "Coincident centres"), as the kernel does
+static void contactNormal(const double* d, double len, double* n) {
+  if (len > 0.0) {
+    for (int i = 0; i < 3; ++i) n[i] = d[i] / len;
+  } else {
+    n[0] = 1.0; n[1] = 0.0; n[2] = 0.0;
+  }
+}
 struct Contact {
   int sphere, obstacle;
   double dist;
@@ -347,10 +356,8 @@ struct CollisionEval {
         ct.sphere = static_cast<int>(s);
         ct.obstacle = o;
         ct.dist = dist;
-        for (int i = 0; i < 3; ++i) {
-          ct.normal[i] = d[i] / len;
-          ct.point[i] = c[i];
-        }
+        contactNormal(d, len, ct.normal);
+        for (int i = 0; i < 3; ++i) ct.point[i] = c[i];
         out.push_back(ct);
       }
     }
@@ -397,8 +404,9 @@ struct CollisionEval {
         const double dist = len - sp.radius - ob[3];
         Vec row(D + 3, 0.0);
         const bool filtered = dist > margin + buffer;  // no expression is ever built for a filtered contact
-        if (!filtered)
-          for (int j = 0; j < D; ++j) row[j] = -(d[0] * J[0][j] + d[1] * J[1][j] + d[2] * J[2][j]) / len;
+        if (!filtered)  // (coincident centres: the normal (1, 0, 0) of contactNormal)
+          for (int j = 0; j < D; ++j)
+            row[j] = len > 0.0 ? -(d[0] * J[0][j] + d[1] * J[1][j] + d[2] * J[2][j]) / len : -J[0][j];
         row[D] = dist;
         row[D + 1] = margin;
         row[D + 2] = filtered ? 0.0 : coeff;
@@ -517,7 +525,7 @@ struct CastCollisionEval {
           ct.sphere = s; ct.obstacle = o; ct.sub = i;
           ct.dist = len - sp.radius - ob[3];
           ct.cc_time = (i + sc) / n;
-          for (int k = 0; k < 3; ++k) ct.normal[k] = d[k] / len;
+          contactNormal(d, len, ct.normal);
           const bool time0 = (i == 0 && sc == 0.0), time1 = discrete_states ? (i == n) : (i == n - 1 && sc == 1.0);
           cd.active = !(ct.dist > margin + buffer) && !(start_fixed && time0) && !(end_fixed && time1);
           ct.g0.assign(D, 0.0);
@@ -839,6 +847,9 @@ TrajProblem buildProblem(const tb200_problem_desc& desc, int b, int cast_cap) {
     obstacles.assign(o, o + desc.n_obstacles * 4);
   }
 
+  // the collision rows of the cost objects come first, then those of the constraints (the objects' OptProb order, the
+  // layout of tb200_convexify_batch)
+  std::vector<std::function<void(const Vec& x, std::vector<Vec>& rows)>> cnt_coll_hooks;
   for (int k = 0; k < desc.n_terms; ++k) {
     const tb200_term& tm = desc.terms[k];
     const bool is_cost = tm.role == TB200_ROLE_COST;
@@ -1014,7 +1025,7 @@ TrajProblem buildProblem(const tb200_problem_desc& desc, int b, int cast_cap) {
             // (two adjacent fixed steps fall into the START_FIXED_END_FREE branch: the reference's throw is unreachable)
             CastCollisionEval e{tp.robot, obstacles, t, D, tm.margin, tm.coeff, tm.margin_buffer, lvs, cur_fixed,
                                 !cur_fixed && next_fixed, cast_cap, tm.evaluator_type == TB200_COLL_LVS_DISCRETE};
-            tp.coll_hooks.push_back([e](const Vec& x, std::vector<Vec>& rows) { e.denseRows(x, rows); });
+            (is_cost ? tp.coll_hooks : cnt_coll_hooks).push_back([e](const Vec& x, std::vector<Vec>& rows) { e.denseRows(x, rows); });
             if (is_cost)
               addCost(std::make_shared<CollisionCost>(calcOf(e)), nm + "_" + std::to_string(t), t);
             else
@@ -1028,7 +1039,7 @@ TrajProblem buildProblem(const tb200_problem_desc& desc, int b, int cast_cap) {
           for (int f = 0; f < tm.n_fixed_steps; ++f) fixed |= (tm.fixed_steps[f] == t);
           if (fixed) continue;
           CollisionEval e{tp.robot, obstacles, t, D, tm.margin, tm.coeff, tm.margin_buffer};
-          tp.coll_hooks.push_back([e](const Vec& x, std::vector<Vec>& rows) { e.denseRows(x, rows); });
+          (is_cost ? tp.coll_hooks : cnt_coll_hooks).push_back([e](const Vec& x, std::vector<Vec>& rows) { e.denseRows(x, rows); });
           if (is_cost)
             addCost(std::make_shared<CollisionCost>(calcOf(e)), nm + "_" + std::to_string(t), t);
           else
@@ -1077,6 +1088,7 @@ TrajProblem buildProblem(const tb200_problem_desc& desc, int b, int cast_cap) {
         throw std::runtime_error("unknown term kind");
     }
   }
+  tp.coll_hooks.insert(tp.coll_hooks.end(), cnt_coll_hooks.begin(), cnt_coll_hooks.end());
   for (auto& c : tp.prob->getCosts()) tp.cost_names.push_back(c->name);
   for (auto& c : tp.prob->getConstraints()) tp.cnt_names.push_back(c->name);
   return tp;

@@ -56,7 +56,8 @@ struct TrajProblem {
   // Hooks for the kernel-level parity tests (fixed dense layout shared with the CUDA path):
   // coefficient-scaled Cartesian error rows (err, jac rows over the term's variables), in term order;
   std::vector<std::function<void(const Vec& x, Vec& err, std::vector<Vec>& jac)>> cart_hooks;
-  // dense candidate collision rows [(sphere, obstacle)] = {grad[D], dist0, margin, coeff or 0 if filtered}
+  // dense candidate collision rows [(sphere, obstacle)] = {grad[D], dist0, margin, coeff or 0 if filtered}: the cost
+  // objects' first, then the constraints', each in term order
   std::vector<std::function<void(const Vec& x, std::vector<Vec>& rows)>> coll_hooks;
 };
 // avoid_singularity: J [6][D] row-major -> its smallest singular value and singular vectors u[6], v[D] (the undefined

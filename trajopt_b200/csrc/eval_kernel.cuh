@@ -787,8 +787,11 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
             // for a filtered contact, collision_terms.cpp:655-691): the other candidates keep a zero gradient.
             if (active) {
               const double cx = cx2[h], cy = cy2[h], cz = cz2[h];
-              const double inv = 1.0 / len2[h];
-              const double nx = dx2[h] * inv, ny = dy2[h] * inv, nz = dz2[h] * inv;  // from the robot sphere towards the obstacle
+              // from the robot sphere towards the obstacle; coincident centres (len 0) take the fixed normal (1, 0, 0)
+              // of the scene frame instead of 0/0 (DESIGN.md section 6, "Coincident centres")
+              const bool coincident = !(len2[h] > 0.0);
+              const double inv = coincident ? 0.0 : 1.0 / len2[h];
+              const double nx = coincident ? 1.0 : dx2[h] * inv, ny = dy2[h] * inv, nz = dz2[h] * inv;
               const double mx = cy * nz - cz * ny, my = cz * nx - cx * nz, mz = cx * ny - cy * nx;  // c x n
               const unsigned jm = ex.sphere_jmask[sl];
 #pragma unroll
@@ -987,7 +990,8 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
           const double wx = cb[0] - ca[0], wy = cb[1] - ca[1], wz = cb[2] - ca[2];
           const double dx = ob.x - (ca[0] + sc * wx), dy = ob.y - (ca[1] + sc * wy), dz = ob.z - (ca[2] + sc * wz);
           const double len = sqrt(dx * dx + dy * dy + dz * dz);
-          const double nxs = dx / len, nys = dy / len, nzs = dz / len;
+          const bool coincident = !(len > 0.0);  // an obstacle centre on the swept segment: the fixed normal (1, 0, 0)
+          const double nxs = coincident ? 1.0 : dx / len, nys = coincident ? 0.0 : dy / len, nzs = coincident ? 0.0 : dz / len;
           const double cc_s = (i_s + sc) / nsub;
           if (lane_c < D) qv[lane_c] = (cc_s == 1.0) ? q1[lane_c] : q0[lane_c] + (q1[lane_c] - q0[lane_c]) * cc_s;
           __syncwarp();
@@ -1064,8 +1068,11 @@ __device__ __forceinline__ void eval_step_impl(const DevProblem& p, const EvalEx
         for (int k = 0; k < ex.n_joint_objs; ++k) slot_j = (ex.joint_obj_idx[k] == i) ? k : slot_j;
         v = sm[S.objv + p.n_coll_objs + slot_j];  // summed in order by a warp of the row phase
       } else if (o.kind == OBJ_CART_POSE) {
+        // rows e = c * err: EQ violation sum |c err|; the ABS cost is sum c |err| (CostFromErrFunc::value applies the
+        // coefficient after the abs, modeling_utils.cpp:143-166), so a negative coefficient gives a negative term
         const double* e = p.cart_err + slot * p.n_cart_rows + o.src_off;
-        for (int r = 0; r < o.n_rows; ++r) v += fabs(e[r]);
+        const DevCartTerm& ct = p.cart_terms[o.term];
+        for (int r = 0; r < o.n_rows; ++r) v += (!is_cnt && ct.coeff[r] < 0.0) ? -fabs(e[r]) : fabs(e[r]);
       } else if (o.kind == OBJ_CART_VEL) {
         const double* e = p.cart_err + slot * p.n_cart_rows + o.src_off;
         for (int r = 0; r < 6; ++r) v += is_cnt ? fmax(e[r], 0.0) : fabs(e[r]);  // INEQ violation | ABS cost
