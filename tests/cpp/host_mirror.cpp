@@ -1,13 +1,12 @@
 // Exercises the C++ host layer (include/trajopt_b200.hpp) the way a caller of the reference writes a problem:
-// ProblemConstructionInfo + TermInfo objects -> ConstructProblem -> OptimizeProblem.  Reads the robot and the
-// per-problem data from a text file written by tests/test_cpp_host.py, builds the configs[2] description and either
-// dumps the flattened POD description (mode "dump", no device needed) or solves it (mode "solve").
+// ProblemConstructionInfo + TermInfo objects -> ConstructProblem -> OptimizeProblem.  Reads the problem file
+// (host_input.hpp), builds the configs[2] description and either dumps the flattened POD description (mode "dump", no
+// device needed) or solves it (mode "solve").
 #include <cstdio>
 #include <fstream>
-#include <iostream>
-
 #include <sstream>
 
+#include "host_input.hpp"
 #include "trajopt_b200_json.hpp"
 
 namespace tb = trajopt_b200;
@@ -15,48 +14,19 @@ using namespace tb::trajopt;
 
 int main(int argc, char** argv) {
   if (argc < 3) return 2;
-  std::ifstream in(argv[1]);
+  HostProblem hp = readProblem(argv[1]);
   const std::string mode = argv[2];
-  int B, T, D, nseg;
-  in >> B >> T >> D >> nseg;
-  auto kin = std::make_shared<RobotModel>();
-  for (int s = 0; s < nseg; ++s) {
-    RobotModel::Joint j;
-    in >> j.parent >> j.type >> j.q_index >> j.origin.xyz[0] >> j.origin.xyz[1] >> j.origin.xyz[2] >> j.origin.wxyz[0] >>
-        j.origin.wxyz[1] >> j.origin.wxyz[2] >> j.origin.wxyz[3] >> j.axis[0] >> j.axis[1] >> j.axis[2] >> j.child_link;
-    kin->joints.push_back(j);
-  }
-  kin->lower.resize(D);
-  kin->upper.resize(D);
-  for (double& v : kin->lower) in >> v;
-  for (double& v : kin->upper) in >> v;
-  int nsph;
-  in >> nsph;
-  for (int s = 0; s < nsph; ++s) {
-    RobotModel::Sphere sp;
-    in >> sp.link >> sp.center[0] >> sp.center[1] >> sp.center[2] >> sp.radius;
-    kin->spheres.push_back(sp);
-  }
-  std::string tool;
-  in >> tool;
-  ProblemConstructionInfo pci;
-  pci.kin = kin;
-  pci.batch = B;
-  pci.basic_info.n_steps = T;
-  pci.basic_info.manip = "right_arm";
-  pci.basic_info.fixed_timesteps = {0};
-  pci.basic_info.convex_solver = tb::sco::modelTypeFromName("OSQP");
+  ProblemConstructionInfo& pci = hp.pci;
+  // JOINT_INTERPOLATED from the first to the last waypoint of the file's trajectories
+  const int B = pci.batch, T = pci.basic_info.n_steps, D = pci.kin->numJoints();
+  tb::DblVec traj;
+  traj.swap(pci.init_info.data);
   pci.init_info.type = InitInfo::JOINT_INTERPOLATED;
-  pci.init_info.start.resize(static_cast<size_t>(B) * D);
-  pci.init_info.data.resize(static_cast<size_t>(B) * D);
-  for (double& v : pci.init_info.start) in >> v;
-  for (double& v : pci.init_info.data) in >> v;
-  std::vector<Pose> goals(B);
-  for (Pose& g : goals) in >> g.xyz[0] >> g.xyz[1] >> g.xyz[2] >> g.wxyz[0] >> g.wxyz[1] >> g.wxyz[2] >> g.wxyz[3];
-  in >> pci.n_obstacles;
-  pci.obstacles.resize(static_cast<size_t>(B) * pci.n_obstacles * 4);
-  for (double& v : pci.obstacles) in >> v;
-  if (!in) { std::fprintf(stderr, "bad input file\n"); return 2; }
+  for (int b = 0; b < B; ++b) {
+    const auto first = traj.begin() + static_cast<size_t>(b) * T * D, last = first + (T - 1) * D;
+    pci.init_info.start.insert(pci.init_info.start.end(), first, first + D);
+    pci.init_info.data.insert(pci.init_info.data.end(), last, last + D);
+  }
 
   if (mode == "json") {  // the description comes from a JSON document in the reference's schema (argv[3])
     try {
@@ -64,7 +34,7 @@ int main(int argc, char** argv) {
       std::stringstream ss;
       ss << jf.rdbuf();
       ProblemConstructionInfo jp;
-      jp.kin = kin;
+      jp.kin = pci.kin;
       jp.batch = B;
       jp.obstacles = pci.obstacles;
       jp.n_obstacles = pci.n_obstacles;
@@ -88,27 +58,7 @@ int main(int argc, char** argv) {
     }
   }
 
-  auto vel = std::make_shared<JointVelTermInfo>();
-  vel->term_type = TT_COST;
-  vel->first_step = 0; vel->last_step = T - 1;
-  auto acc = std::make_shared<JointAccTermInfo>();
-  acc->term_type = TT_COST;
-  acc->first_step = 0; acc->last_step = T - 1;
-  pci.cost_infos = {vel, acc};
-  auto pose = std::make_shared<CartPoseTermInfo>();
-  pose->term_type = TT_CNT;
-  pose->timestep = T - 1;
-  pose->source_frame = tool;
-  pose->target = goals;
-  auto coll = std::make_shared<CollisionTermInfo>();
-  coll->term_type = TT_CNT;
-  coll->first_step = 0; coll->last_step = T - 1;
-  coll->fixed_steps = {0};
-  coll->evaluator_type = TB200_COLL_DISCRETE;
-  coll->collision_margin = 0.02; coll->collision_coeff = 20.0; coll->collision_margin_buffer = 0.01;
-  coll->longest_valid_segment_length = 0.5;
-  pci.cnt_infos = {pose, coll};
-
+  appendConfig2Terms(hp);
   try {
     if (mode == "dump") {
       auto fp = FlattenProblem(pci);

@@ -2,17 +2,17 @@
 //   sqp_log_host synth <dir>          no device: a synthetic log (two problems, written below) is replayed through
 //                                     ReplayCallbacks, printing one "cb" line per callback, and written by WriteLogResults
 //                                     into <dir>/<problem>
-//   sqp_log_host solve <input> <dir>  configs[2] from the input file (the layout of multi_start_host.cpp without groups)
-//                                     with log_results on: OptimizeWithParams with a printing callback and a
-//                                     WriteCallback into <dir>/write.csv; prints the callbacks and the final results of
-//                                     the logged and the plain solve
+//   sqp_log_host solve <input> <dir>  configs[2] on the problem file (host_input.hpp) with log_results on:
+//                                     OptimizeWithParams with a printing callback and a WriteCallback into
+//                                     <dir>/write.csv; prints the callbacks and the final results of the logged and
+//                                     the plain solve
 //   sqp_log_host fk <input>           no device: RobotFK of every waypoint of trajectory 0 ("fk t joint R[9] p[3]")
 //   sqp_log_host write <input> <csv>  no device: WriteCallback over the input's robot with synthetic names and results
 //                                     (x = trajectory 0), called twice
 #include <cstdio>
 #include <fstream>
 
-#include "trajopt_b200.hpp"
+#include "host_input.hpp"
 
 namespace tb = trajopt_b200;
 using namespace tb::trajopt;
@@ -102,47 +102,13 @@ int main(int argc, char** argv) {
       }
       return 0;
     }
-    std::ifstream in(argv[2]);
-    int B, T, D, nseg;
-    in >> B >> T >> D >> nseg;
-    auto kin = std::make_shared<RobotModel>();
-    for (int s = 0; s < nseg; ++s) {
-      RobotModel::Joint j;
-      in >> j.parent >> j.type >> j.q_index >> j.origin.xyz[0] >> j.origin.xyz[1] >> j.origin.xyz[2] >> j.origin.wxyz[0] >>
-          j.origin.wxyz[1] >> j.origin.wxyz[2] >> j.origin.wxyz[3] >> j.axis[0] >> j.axis[1] >> j.axis[2] >> j.child_link;
-      kin->joints.push_back(j);
-    }
-    kin->lower.resize(D);
-    kin->upper.resize(D);
-    for (double& v : kin->lower) in >> v;
-    for (double& v : kin->upper) in >> v;
-    int nsph;
-    in >> nsph;
-    for (int s = 0; s < nsph; ++s) {
-      RobotModel::Sphere sp;
-      in >> sp.link >> sp.center[0] >> sp.center[1] >> sp.center[2] >> sp.radius;
-      kin->spheres.push_back(sp);
-    }
-    std::string tool;
-    in >> tool;
-    ProblemConstructionInfo pci;
-    pci.kin = kin;
-    pci.batch = B;
-    pci.basic_info.n_steps = T;
-    pci.basic_info.fixed_timesteps = {0};
-    pci.init_info.type = InitInfo::GIVEN_TRAJ;
-    pci.init_info.data.resize(static_cast<size_t>(B) * T * D);
-    for (double& v : pci.init_info.data) in >> v;
-    std::vector<Pose> goals(B);
-    for (Pose& g : goals) in >> g.xyz[0] >> g.xyz[1] >> g.xyz[2] >> g.wxyz[0] >> g.wxyz[1] >> g.wxyz[2] >> g.wxyz[3];
-    in >> pci.n_obstacles;
-    pci.obstacles.resize(static_cast<size_t>(B) * pci.n_obstacles * 4);
-    for (double& v : pci.obstacles) in >> v;
-    if (!in) { std::fprintf(stderr, "bad input file\n"); return 2; }
+    HostProblem hp = readProblem(argv[2]);
+    ProblemConstructionInfo& pci = hp.pci;
+    const int T = pci.basic_info.n_steps, D = pci.kin->numJoints();
     const double* x0 = pci.init_info.data.data();
     if (mode == "fk") {
       for (int t = 0; t < T; ++t) {
-        const std::vector<Frame> fr = RobotFK(*kin, x0 + static_cast<size_t>(t) * D);
+        const std::vector<Frame> fr = RobotFK(*pci.kin, x0 + static_cast<size_t>(t) * D);
         for (size_t j = 0; j < fr.size(); ++j) {
           std::printf("fk %d %zu", t, j);
           for (double v : fr[j].R) std::printf(" %.17g", v);
@@ -154,7 +120,7 @@ int main(int argc, char** argv) {
     }
     if (mode == "write") {
       auto file = std::make_shared<std::ofstream>(argv[3]);
-      Callback cb = WriteCallback(file, kin, {"joint_vel", "joint_acc"}, {"cart_pose", "collision_3"});
+      Callback cb = WriteCallback(file, pci.kin, {"joint_vel", "joint_acc"}, {"cart_pose", "collision_3"});
       tb::sco::OptResults r;
       r.x.assign(x0, x0 + static_cast<size_t>(T) * D);
       r.cost_vals = {1.5, 0.0625};
@@ -165,25 +131,7 @@ int main(int argc, char** argv) {
       return 0;
     }
     if (mode != "solve" || argc < 4) return 2;
-    auto vel = std::make_shared<JointVelTermInfo>();
-    vel->term_type = TT_COST;
-    vel->first_step = 0; vel->last_step = T - 1;
-    auto acc = std::make_shared<JointAccTermInfo>();
-    acc->term_type = TT_COST;
-    acc->first_step = 0; acc->last_step = T - 1;
-    pci.cost_infos = {vel, acc};
-    auto pose = std::make_shared<CartPoseTermInfo>();
-    pose->term_type = TT_CNT;
-    pose->timestep = T - 1;
-    pose->source_frame = tool;
-    pose->target = goals;
-    auto coll = std::make_shared<CollisionTermInfo>();
-    coll->term_type = TT_CNT;
-    coll->first_step = 0; coll->last_step = T - 1;
-    coll->fixed_steps = {0};
-    coll->evaluator_type = TB200_COLL_DISCRETE;
-    coll->collision_margin = 0.02; coll->collision_coeff = 20.0; coll->collision_margin_buffer = 0.01;
-    pci.cnt_infos = {pose, coll};
+    appendConfig2Terms(hp);
     pci.opt_info.log_results = true;
     pci.opt_info.log_dir = argv[3];
     TrajOptProb::Ptr prob = ConstructProblem(pci);

@@ -2,15 +2,14 @@
 oracle's term (one-sided Jacobi SVD, err, forward-difference gradient) against numpy, and on the GPU (-m gpu) the
 device's rows, QP and SQP against the oracle."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
+import cpp_host
 from trajopt_b200 import api, capi, json_io, problems, robots
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 _dbl_p = C.POINTER(C.c_double)
 _i32_p = C.POINTER(C.c_int32)
 
@@ -393,14 +392,7 @@ def test_sqp_log_matches_the_model(oracle, name):
 
 @pytest.fixture(scope="module")
 def host_bin(tmp_path_factory):
-    capi.load_library()  # the CUDA build must exist (no GPU needed to load it)
-    csrc = os.path.join(ROOT, "trajopt_b200", "csrc")
-    out = str(tmp_path_factory.mktemp("ash") / "avoid_singularity_host")
-    cmd = ["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-Werror", "-I", os.path.join(ROOT, "include"),
-           os.path.join(ROOT, "tests", "cpp", "avoid_singularity_host.cpp"), "-o", out, "-L", csrc, "-ltrajopt_b200",
-           "-Wl,-rpath," + csrc, "-Wl,--allow-shlib-undefined"]
-    subprocess.run(cmd, check=True)
-    return out
+    return cpp_host.build(tmp_path_factory, "avoid_singularity_host")
 
 
 @pytest.mark.parametrize("mode,rc,text", [

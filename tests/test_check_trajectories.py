@@ -15,11 +15,11 @@ import subprocess
 import numpy as np
 import pytest
 
+import cpp_host
 from trajopt_b200 import capi, problems, robots
 from test_reference_json import _load
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "trajopt_b200", "csrc")
 TYPES = [capi.COLL_DISCRETE, capi.COLL_LVS_DISCRETE, capi.COLL_CONTINUOUS, capi.COLL_LVS_CONTINUOUS]
 
 
@@ -45,14 +45,11 @@ class CheckOracle:
 
 @pytest.fixture(scope="module")
 def chk(oracle, tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("chk") / "libcheck_oracle.so")
     lib = os.path.join(ROOT, "oracle", "liboracle.so")
     # the oracle's own flags (oracle/Makefile)
-    cmd = ["g++", "-std=c++17", "-O3", "-march=x86-64-v3", "-fopenmp", "-fPIC", "-DNDEBUG", "-shared",
-           "-I", os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tests", "cpp", "check_oracle.cpp"), lib,
-           "-Wl,-rpath," + os.path.dirname(lib), "-o", out]
-    subprocess.run(cmd, check=True)
-    return CheckOracle(out)
+    flags = ("-O3", "-march=x86-64-v3", "-fopenmp", "-DNDEBUG", "-I", os.path.join(ROOT, "oracle"), lib,
+             "-Wl,-rpath," + os.path.dirname(lib))
+    return CheckOracle(cpp_host.build(tmp_path_factory, "check_oracle", shared=True, extra=flags))
 
 
 # ---- plain-numpy restatement -------------------------------------------------------------------------------------
@@ -363,27 +360,7 @@ def test_refusals():
 # ---- C++ host layer ------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def host_bin(tmp_path_factory):
-    capi.load_library()  # the CUDA build must exist (no GPU needed to load it)
-    out = str(tmp_path_factory.mktemp("chkcpp") / "check_host")
-    cmd = ["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-I", os.path.join(ROOT, "include"),
-           os.path.join(ROOT, "tests", "cpp", "check_host.cpp"), "-o", out, "-L", CSRC, "-ltrajopt_b200",
-           "-Wl,-rpath," + CSRC, "-Wl,--allow-shlib-undefined"]
-    subprocess.run(cmd, check=True)
-    return out
-
-
-def _write_input(path, d, x, type, lvs, margin):
-    rob = d.robot_spec
-    with open(path, "w") as f:
-        f.write(f"{d.B} {d.T} {d.D} {len(rob['segments'])} {type} {lvs!r} {margin!r}\n")
-        for s in rob["segments"]:
-            f.write(" ".join(repr(v) for v in [s.parent, s.joint_type, s.q_index, *s.origin_xyz, *s.origin_wxyz, *s.axis]) + "\n")
-        f.write(" ".join(repr(float(v)) for v in [*rob["lower"], *rob["upper"]]) + "\n")
-        f.write(f"{len(rob['spheres'])}\n")
-        for s in rob["spheres"]:
-            f.write(" ".join(repr(v) for v in [s.segment, *s.center, s.radius]) + "\n")
-        f.write(" ".join(repr(float(v)) for v in x.ravel()) + "\n")
-        f.write(f"{d.obstacles.shape[1]}\n" + " ".join(repr(float(v)) for v in d.obstacles.ravel()) + "\n")
+    return cpp_host.build(tmp_path_factory, "check_host")
 
 
 def test_host_program_builds(host_bin):
@@ -395,11 +372,11 @@ def test_host_program_builds(host_bin):
 def test_cpp_layer_returns_the_c_abi_values(host_bin, tmp_path, type):
     from trajopt_b200 import api
     d, x, lvs, margin = case("cfg2")
-    path = str(tmp_path / "in.txt")
-    _write_input(path, d, x, type, lvs, margin)
-    out = subprocess.run([host_bin, path], capture_output=True, text=True, check=True).stdout.split("\n")
     # (the same description without terms: which fixed segments the host folds, and so the FK's products, match)
-    want = api.check(capi.ProblemDesc(d.robot_spec, d.T, [], x, obstacles=d.obstacles), x, type=type, lvs=lvs, margin=margin)
+    e = capi.ProblemDesc(d.robot_spec, d.T, [], x, obstacles=d.obstacles)
+    out = subprocess.run([host_bin, cpp_host.write_problem(tmp_path / "in.txt", e), str(type), repr(lvs), repr(margin)],
+                         capture_output=True, text=True, check=True).stdout.split("\n")
+    want = api.check(e, x, type=type, lvs=lvs, margin=margin)
     for b in range(d.B):
         v = out[b].split()
         assert int(v[0]) == int(want["in_collision"][b]) and int(v[1]) == want["first_slot"][b]

@@ -2,57 +2,27 @@
 OptimizeProblem under the reference's names) against the Python mirror of the same C ABI.
 CPU: it compiles, flattens configs[2] to the byte-identical POD description, and fails loudly without a device.
 GPU (-m gpu): solving through it gives the results of the Python path."""
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
+import cpp_host
 from trajopt_b200 import api, capi, problems, robots  # noqa: F401
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "trajopt_b200", "csrc")
 
 
 @pytest.fixture(scope="module")
 def host_bin(tmp_path_factory):
-    capi.load_library()  # the CUDA build must exist (no GPU needed to load it)
-    out = str(tmp_path_factory.mktemp("cpp") / "host_mirror")
-    cmd = ["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-I", os.path.join(ROOT, "include"),
-           os.path.join(ROOT, "tests", "cpp", "host_mirror.cpp"), "-o", out, "-L", CSRC, "-ltrajopt_b200",
-           "-Wl,-rpath," + CSRC, "-Wl,--allow-shlib-undefined"]
-    subprocess.run(cmd, check=True)
-    return out
-
-
-def _write_input(path, d, q0, q1):
-    robot = d.robot_spec
-    names = [f"link{i}" for i in range(len(robot["segments"]))]
-    with open(path, "w") as f:
-        f.write(f"{d.B} {d.T} {d.D} {len(robot['segments'])}\n")
-        for i, s in enumerate(robot["segments"]):
-            vals = [s.parent, s.joint_type, s.q_index, *s.origin_xyz, *s.origin_wxyz, *s.axis]
-            f.write(" ".join(repr(float(v)) if isinstance(v, float) else str(v) for v in vals) + f" {names[i]}\n")
-        f.write(" ".join(repr(float(v)) for v in robot["lower"]) + "\n")
-        f.write(" ".join(repr(float(v)) for v in robot["upper"]) + "\n")
-        f.write(f"{len(robot['spheres'])}\n")
-        for sp in robot["spheres"]:
-            f.write(f"{names[sp.segment]} " + " ".join(repr(float(v)) for v in (*sp.center, sp.radius)) + "\n")
-        f.write(names[robot["tool"]] + "\n")
-        for arr in (q0, q1, d.cart_targets.reshape(d.B, 7)):
-            f.write(" ".join(repr(float(v)) for v in arr.ravel()) + "\n")
-        f.write(f"{d.obstacles.shape[1]}\n" + " ".join(repr(float(v)) for v in d.obstacles.ravel()) + "\n")
+    return cpp_host.build(tmp_path_factory, "host_mirror")
 
 
 def _case(tmp_path):
     d = problems.config2(B=3, T=10)
-    q0, q1 = d.init_traj[:, 0].copy(), d.init_traj[:, -1].copy()
-    path = str(tmp_path / "in.txt")
-    _write_input(path, d, q0, q1)
-    return d, path
+    return d, cpp_host.write_problem(tmp_path / "in.txt", d)
 
 
 def test_cpp_host_flattens_to_the_same_description(host_bin, tmp_path):
+    """configs[2] as tests/cpp/host_input.hpp writes it, for every host program that solves it."""
     d, path = _case(tmp_path)
     out = subprocess.run([host_bin, path, "dump"], check=True, capture_output=True, text=True).stdout.splitlines()
     assert out[0] == f"n_terms {len(d.terms)} n_cart_targets 1 n_fixed 1"

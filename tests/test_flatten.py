@@ -4,23 +4,16 @@ quadratic objective of each description hash to pinned FNV-1a digests.  These ar
 change to the flattening that alters any of them fails here on any machine.  The digests were taken from the library
 as it was before the stage moved into its own header."""
 import ctypes as C
-import os
-import subprocess
 
 import pytest
 
+import cpp_host
 from trajopt_b200 import capi, problems
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
 def flat(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("flatten") / "flatten_digest.so")
-    cmd = ["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-shared", "-fPIC", "-I", os.path.join(ROOT, "include"),
-           os.path.join(ROOT, "tests", "cpp", "flatten_digest.cpp"), "-o", out]
-    subprocess.run(cmd, check=True)
-    lib = C.CDLL(out)
+    lib = C.CDLL(cpp_host.build(tmp_path_factory, "flatten_digest", shared=True))
     lib.flatten_digest.argtypes = [C.POINTER(capi.ProblemDescC), C.POINTER(C.c_uint64), C.c_char_p, C.c_int]
     lib.flatten_digest.restype = C.c_int
     return lib

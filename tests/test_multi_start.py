@@ -15,10 +15,9 @@ import subprocess
 import numpy as np
 import pytest
 
+import cpp_host
 from trajopt_b200 import api, capi, problems, sharding
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "trajopt_b200", "csrc")
 _dbl_p = C.POINTER(C.c_double)
 _i32_p = C.POINTER(C.c_int32)
 RESULT_KEYS = ("status", "n_qp_solves", "n_func_evals", "n_admm_iters", "x", "total_cost", "cost_vals", "cnt_viols")
@@ -27,13 +26,7 @@ RESULT_KEYS = ("status", "n_qp_solves", "n_func_evals", "n_admm_iters", "x", "to
 # ---------------------------------------------------------------------------------------------------------- fixtures
 @pytest.fixture(scope="module")
 def host_bin(tmp_path_factory):
-    capi.load_library()  # the CUDA build must exist (no GPU needed to load it)
-    out = str(tmp_path_factory.mktemp("mscpp") / "multi_start_host")
-    cmd = ["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-I", os.path.join(ROOT, "include"),
-           os.path.join(ROOT, "tests", "cpp", "multi_start_host.cpp"), "-o", out, "-L", CSRC, "-ltrajopt_b200",
-           "-Wl,-rpath," + CSRC, "-Wl,--allow-shlib-undefined"]
-    subprocess.run(cmd, check=True)
-    return out
+    return cpp_host.build(tmp_path_factory, "multi_start_host")
 
 
 def seeded(make, n_seeds, group_stop=0, seed=7, spread=0.6):
@@ -220,30 +213,10 @@ def test_two_rank_gloo_never_splits_a_group(oracle, tmp_path):
     assert sizes == [4, 2]
 
 
-def _write_input(path, d):
-    robot = d.robot_spec
-    names = [f"link{i}" for i in range(len(robot["segments"]))]
-    with open(path, "w") as f:
-        f.write(f"{d.B} {d.T} {d.D} {len(robot['segments'])} {d.c.group_size} {d.c.group_stop}\n")
-        for i, s in enumerate(robot["segments"]):
-            vals = [s.parent, s.joint_type, s.q_index, *s.origin_xyz, *s.origin_wxyz, *s.axis]
-            f.write(" ".join(repr(float(v)) if isinstance(v, float) else str(v) for v in vals) + f" {names[i]}\n")
-        f.write(" ".join(repr(float(v)) for v in robot["lower"]) + "\n")
-        f.write(" ".join(repr(float(v)) for v in robot["upper"]) + "\n")
-        f.write(f"{len(robot['spheres'])}\n")
-        for sp in robot["spheres"]:
-            f.write(f"{names[sp.segment]} " + " ".join(repr(float(v)) for v in (*sp.center, sp.radius)) + "\n")
-        f.write(names[robot["tool"]] + "\n")
-        for arr in (d.init_traj, d.cart_targets.reshape(d.B, 7)):
-            f.write(" ".join(repr(float(v)) for v in arr.ravel()) + "\n")
-        f.write(f"{d.obstacles.shape[1]}\n" + " ".join(repr(float(v)) for v in d.obstacles.ravel()) + "\n")
-
-
 def test_cpp_layer_flattens_the_groups(host_bin, tmp_path):
     d = seeded(lambda: problems.config2(B=3, T=10), 4, group_stop=1)
-    path = str(tmp_path / "in.txt")
-    _write_input(path, d)
-    out = subprocess.run([host_bin, path, "dump"], check=True, capture_output=True, text=True).stdout.split()
+    out = subprocess.run([host_bin, cpp_host.write_problem(tmp_path / "in.txt", d), "dump", str(d.c.group_size),
+                          str(d.c.group_stop)], check=True, capture_output=True, text=True).stdout.split()
     assert out == ["batch", "12", "group_size", "4", "group_stop", "1"]
 
 
@@ -421,9 +394,8 @@ def test_device_groups_with_a_time_limit(runs):
 
 
 def _cpp_solve(host_bin, tmp_path, d):
-    path = str(tmp_path / "in.txt")
-    _write_input(path, d)
-    out = subprocess.run([host_bin, path, "solve"], check=True, capture_output=True, text=True).stdout.splitlines()
+    out = subprocess.run([host_bin, cpp_host.write_problem(tmp_path / "in.txt", d), "solve", str(d.c.group_size),
+                          str(d.c.group_stop)], check=True, capture_output=True, text=True).stdout.splitlines()
     rows = [line.split() for line in out]
     assert len(rows) == d.B // d.c.group_size and all(v[0] == "problem" for v in rows)
     return [(int(v[1]), int(v[2]), float(v[3]), np.array(v[4:], int)) for v in rows]

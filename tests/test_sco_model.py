@@ -4,27 +4,17 @@ exactly as they are written against trajopt_sco.  CPU: the canonical QP the mode
 updateConstraints, osqp_interface.cpp:170-281) and its bookkeeping.  GPU: the cases solved, and the general QP entry
 point against the CPU oracle's OSQP-equivalent solver on random QPs."""
 import ctypes as C
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
-import __graft_entry__ as entry
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "trajopt_b200", "csrc")
+import cpp_host
 
 
 @pytest.fixture(scope="module")
 def exe(tmp_path_factory):
-    entry.build()
-    out = str(tmp_path_factory.mktemp("cpp") / "sco_model")
-    cmd = ["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-I", os.path.join(ROOT, "include"),
-           os.path.join(ROOT, "tests", "cpp", "sco_model.cpp"), "-o", out, "-L", CSRC, "-ltrajopt_b200",
-           "-Wl,-rpath," + CSRC, "-lpthread"]
-    subprocess.run(cmd, check=True)
-    return out
+    return cpp_host.build(tmp_path_factory, "sco_model")
 
 
 def test_model_assembles_the_canonical_qp(exe):

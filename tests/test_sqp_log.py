@@ -14,23 +14,17 @@ from fractions import Fraction
 import numpy as np
 import pytest
 
+import cpp_host
 from trajopt_b200 import api, capi, problems
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "trajopt_b200", "csrc")
 _dbl_p = C.POINTER(C.c_double)
 _i32_p = C.POINTER(C.c_int32)
 
 
 @pytest.fixture(scope="module")
 def host_bin(tmp_path_factory):
-    capi.load_library()  # the CUDA build must exist (no GPU needed to load it)
-    out = str(tmp_path_factory.mktemp("sqplog") / "sqp_log_host")
-    cmd = ["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-Werror", "-I", os.path.join(ROOT, "include"),
-           os.path.join(ROOT, "tests", "cpp", "sqp_log_host.cpp"), "-o", out, "-L", CSRC, "-ltrajopt_b200",
-           "-Wl,-rpath," + CSRC, "-Wl,--allow-shlib-undefined"]
-    subprocess.run(cmd, check=True)
-    return out
+    return cpp_host.build(tmp_path_factory, "sqp_log_host")
 
 
 # ---------------------------------------------------------------------------------------------------------------- CPU
@@ -356,32 +350,11 @@ def test_group_stop_ends_the_stopped_seeds_logs():
         assert L["ended"][b, n - 1] == -1  # its last record is its last QP; the stop came at the next iteration top
 
 
-def _write_input(path, d):
-    robot = d.robot_spec
-    names = [f"link{i}" for i in range(len(robot["segments"]))]
-    with open(path, "w") as f:
-        f.write(f"{d.B} {d.T} {d.D} {len(robot['segments'])}\n")
-        for i, s in enumerate(robot["segments"]):
-            vals = [s.parent, s.joint_type, s.q_index, *s.origin_xyz, *s.origin_wxyz, *s.axis]
-            f.write(" ".join(repr(float(v)) if isinstance(v, float) else str(v) for v in vals) + f" {names[i]}\n")
-        f.write(" ".join(repr(float(v)) for v in robot["lower"]) + "\n")
-        f.write(" ".join(repr(float(v)) for v in robot["upper"]) + "\n")
-        f.write(f"{len(robot['spheres'])}\n")
-        for sp in robot["spheres"]:
-            f.write(f"{names[sp.segment]} " + " ".join(repr(float(v)) for v in (*sp.center, sp.radius)) + "\n")
-        f.write(f"{names[robot['tool']]}\n")
-        f.write(" ".join(repr(float(v)) for v in d.init_traj.ravel()) + "\n")
-        f.write(" ".join(repr(float(v)) for v in d.cart_targets[:, 0].ravel()) + "\n")
-        f.write(f"{d.obstacles.shape[1]}\n" + " ".join(repr(float(v)) for v in d.obstacles.ravel()) + "\n")
-
-
 @pytest.mark.gpu
 def test_cpp_callbacks_and_log_results(host_bin, tmp_path):
     d = problems.config2(B=4, T=12)
-    path = str(tmp_path / "in.txt")
-    _write_input(path, d)
-    out = subprocess.run([host_bin, "solve", path, str(tmp_path / "logs")], check=True, capture_output=True,
-                         text=True).stdout.splitlines()
+    out = subprocess.run([host_bin, "solve", cpp_host.write_problem(tmp_path / "in.txt", d), str(tmp_path / "logs")],
+                         check=True, capture_output=True, text=True).stdout.splitlines()
     rows = [line.split() for line in out]
     final = {int(v[1]): v[2:] for v in rows if v[0] == "final"}
     plain = {int(v[1]): v[2:] for v in rows if v[0] == "plain"}
@@ -452,18 +425,12 @@ def test_log_model_is_the_oracle_driver(oracle, name):
         assert L["x"][b, acc[-1]].tobytes() == ref["x"][b].ravel().tobytes()
 
 
-def _write_input_file(tmp_path, d):
-    path = str(tmp_path / "in.txt")
-    _write_input(path, d)
-    return path
-
-
 @pytest.mark.parametrize("make", [lambda: problems.config2(B=1, T=12), lambda: problems.config4(B=1, T=6)])
 def test_host_fk_is_the_oracle_fk(oracle, host_bin, tmp_path, make):
     """RobotFK of the C++ header restates the oracle's Robot::fk: the same frames, to the last bits."""
     d = make()
-    out = subprocess.run([host_bin, "fk", _write_input_file(tmp_path, d)], check=True, capture_output=True,
-                         text=True).stdout.splitlines()
+    out = subprocess.run([host_bin, "fk", cpp_host.write_problem(tmp_path / "in.txt", d)], check=True,
+                         capture_output=True, text=True).stdout.splitlines()
     S = len(d.robot_spec["segments"])
     got = np.array([[float(t) for t in line.split()[3:]] for line in out]).reshape(d.T, S, 12)
     for t in range(d.T):
@@ -505,7 +472,7 @@ def test_write_callback_csv_layout(oracle, host_bin, tmp_path):
     constraint values), and an empty line; numbers as operator<< prints them (%g)."""
     d = problems.config2(B=1, T=5)
     csv = str(tmp_path / "w.csv")
-    subprocess.run([host_bin, "write", _write_input_file(tmp_path, d), csv], check=True)
+    subprocess.run([host_bin, "write", cpp_host.write_problem(tmp_path / "in.txt", d), csv], check=True)
     segs = d.robot_spec["segments"]
     names = [f"link{i}" for i in range(len(segs))]
     cols = {s.q_index: names[i] for i, s in enumerate(segs) if s.joint_type != capi.JOINT_FIXED}

@@ -13,10 +13,10 @@ import subprocess
 import numpy as np
 import pytest
 
+import cpp_host
 from trajopt_b200 import api, capi, problems, sharding
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "trajopt_b200", "csrc")
 RESULT_KEYS = ("x", "status", "total_cost", "cost_vals", "cnt_viols", "n_qp_solves", "n_func_evals", "n_admm_iters")
 DBL_MAX = np.finfo(np.float64).max
 
@@ -63,7 +63,7 @@ def test_ctypes_mirror_matches_the_header(tmp_path):
     src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "trajopt_b200.h"\n'
                    'int main(void) { printf("%zu %zu %zu\\n", offsetof(tb200_problem_desc, sqp_per_traj), '
                    'sizeof(tb200_problem_desc), sizeof(tb200_sqp_params)); return 0; }\n')
-    exe = str(tmp_path / "layout")
+    exe = str(tmp_path / "layout")  # (a C compile of the header, not a tests/cpp program)
     subprocess.run(["gcc", "-std=c99", "-Wall", "-I", os.path.join(ROOT, "include"), str(src), "-o", exe, "-lm"], check=True)
     off, size, row = map(int, subprocess.run([exe], check=True, capture_output=True, text=True).stdout.split())
     assert off == capi.ProblemDescC.sqp_per_traj.offset
@@ -153,13 +153,7 @@ def test_sweep_shapes():
 
 @pytest.fixture(scope="module")
 def host_bin(tmp_path_factory):
-    capi.load_library()  # the CUDA build must exist (no GPU needed to load it)
-    out = str(tmp_path_factory.mktemp("sqpcpp") / "sqp_params_per_traj_host")
-    cmd = ["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-I", os.path.join(ROOT, "include"),
-           os.path.join(ROOT, "tests", "cpp", "sqp_params_per_traj_host.cpp"), "-o", out, "-L", CSRC, "-ltrajopt_b200",
-           "-Wl,-rpath," + CSRC, "-Wl,--allow-shlib-undefined"]
-    subprocess.run(cmd, check=True)
-    return out
+    return cpp_host.build(tmp_path_factory, "sqp_params_per_traj_host")
 
 
 def test_cpp_rows_are_checked_and_in_order(host_bin):
@@ -289,9 +283,8 @@ def test_setters_replace_and_clear_the_table(host_bin, tmp_path):
                 for t, s, m in ((0.1, 0.1, 50), (0.02, 0.5, 8), (0.3, 0.1, 30), (0.05, 0.3, 50))]
     g = problems.with_seeds(problems.config2(B=3, T=20), 4, np.random.default_rng(2), 0.5)
     want = api.Problem(with_table(g, [cpp_sets[b % 4] for b in range(g.B)])).solve()
-    path = str(tmp_path / "in.txt")
-    _write_input(path, g)
-    out = subprocess.run([host_bin, "solve", path, "4"], check=True, capture_output=True, text=True).stdout.splitlines()
+    out = subprocess.run([host_bin, "solve", cpp_host.write_problem(tmp_path / "in.txt", g), "4", str(g.c.group_size),
+                          str(g.c.group_stop)], check=True, capture_output=True, text=True).stdout.splitlines()
     assert out[0] == "throws"
     trajs = [line.split()[1:] for line in out[1:1 + g.B]]
     for b, (st, cost, nqp, nfe) in enumerate(trajs):
@@ -299,26 +292,6 @@ def test_setters_replace_and_clear_the_table(host_bin, tmp_path):
             (want["status"][b], want["total_cost"][b], want["n_qp_solves"][b], want["n_func_evals"][b])
     probs = [line.split()[1:] for line in out[1 + g.B:]]
     assert len(probs) == g.B // 4
-
-
-def _write_input(path, d):
-    """The description for tests/cpp/sqp_params_per_traj_host.cpp (the format of multi_start_host.cpp)."""
-    robot = d.robot_spec
-    names = [f"link{i}" for i in range(len(robot["segments"]))]
-    with open(path, "w") as f:
-        f.write(f"{d.B} {d.T} {d.D} {len(robot['segments'])} {d.c.group_size} {d.c.group_stop}\n")
-        for i, s in enumerate(robot["segments"]):
-            vals = [s.parent, s.joint_type, s.q_index, *s.origin_xyz, *s.origin_wxyz, *s.axis]
-            f.write(" ".join(repr(float(v)) if isinstance(v, float) else str(v) for v in vals) + f" {names[i]}\n")
-        f.write(" ".join(repr(float(v)) for v in robot["lower"]) + "\n")
-        f.write(" ".join(repr(float(v)) for v in robot["upper"]) + "\n")
-        f.write(f"{len(robot['spheres'])}\n")
-        for sp in robot["spheres"]:
-            f.write(f"{names[sp.segment]} " + " ".join(repr(float(v)) for v in (*sp.center, sp.radius)) + "\n")
-        f.write(names[robot["tool"]] + "\n")
-        for arr in (d.init_traj, d.cart_targets.reshape(d.B, 7)):
-            f.write(" ".join(repr(float(v)) for v in arr.ravel()) + "\n")
-        f.write(f"{d.obstacles.shape[1]}\n" + " ".join(repr(float(v)) for v in d.obstacles.ravel()) + "\n")
 
 
 @pytest.mark.gpu

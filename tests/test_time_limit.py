@@ -7,17 +7,15 @@ rule ("stop at the first iteration top with n_qp_solves >= budget") makes a time
 CPU: defaults, both JSON readers, the CPU model at max_time 0 / DBL_MAX.  GPU (-m gpu): the device against it."""
 import ctypes as C
 import json
-import os
 import subprocess
 import sys
 
 import numpy as np
 import pytest
 
+import cpp_host
 from trajopt_b200 import api, capi, json_io, problems
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "trajopt_b200", "csrc")
 DBL_MAX = sys.float_info.max
 _dbl_p = C.POINTER(C.c_double)
 _i32_p = C.POINTER(C.c_int32)
@@ -25,13 +23,7 @@ _i32_p = C.POINTER(C.c_int32)
 
 @pytest.fixture(scope="module")
 def host_bin(tmp_path_factory):
-    capi.load_library()  # the CUDA build must exist (no GPU needed to load it)
-    out = str(tmp_path_factory.mktemp("tlcpp") / "time_limit_host")
-    cmd = ["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", "-I", os.path.join(ROOT, "include"),
-           os.path.join(ROOT, "tests", "cpp", "time_limit_host.cpp"), "-o", out, "-L", CSRC, "-ltrajopt_b200",
-           "-Wl,-rpath," + CSRC, "-Wl,--allow-shlib-undefined"]
-    subprocess.run(cmd, check=True)
-    return out
+    return cpp_host.build(tmp_path_factory, "time_limit_host")
 
 
 def _costs_only(d):
