@@ -1,0 +1,3 @@
+#define TB200_INST_D 11
+#define TB200_INST_SING 1
+#include "eval_inst.cuh"

@@ -1,0 +1,4 @@
+#define TB200_INST_D 1
+#define TB200_INST_PAIR 0
+#define TB200_INST_SING 1
+#include "solve_inst.cuh"

@@ -1,0 +1,3 @@
+#define TB200_INST_D 4
+#define TB200_INST_PAIR 0
+#include "solve_inst.cuh"

@@ -167,7 +167,7 @@ int planLayout(const tb200_problem_desc& d, const FlatProblem& F, tb200_problem&
 
   const EvalSmem es = eval_smem_layout(T, D, dp.L, dp.n_coll_objs, dp.n_coll_objs * dp.coll_words, dp.S, ex.n_joint_objs,
                                        ex.n_vel_objs, ex.cast, ex.cast_cap, dp.n_costs + dp.n_cnts, ex.n_sing_objs);
-  P.pair_rows = (CN > std::max(D, 3));
+  P.pair_rows = F.has_vel || F.has_cast;  // (at one joint such rows still fit the 3 padded coefficients of a row)
   P.eval_smem = static_cast<size_t>(es.total) * sizeof(double);
   const bool factor_global = D > 8;  // = FG of qp_step: blocks of 2*D > 16 never fit
   const QpSmem qs = qp_smem_layout(N, 2 * D, dp.row_stride, CN, dp.max_rows, factor_global);

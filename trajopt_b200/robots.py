@@ -114,6 +114,126 @@ def spherebot():
                 tool=2)
 
 
+def _copy(robot, **changes):
+    out = dict(robot, segments=[Segment.from_buffer_copy(s) for s in robot["segments"]],
+               spheres=[Sphere.from_buffer_copy(s) for s in robot["spheres"]], lower=list(robot["lower"]),
+               upper=list(robot["upper"]), link_names=list(robot["link_names"]))
+    out.update(changes)
+    return out
+
+
+def with_joints_fixed(robot, links):
+    """`robot` with the joints of the segments named in `links` held FIXED at 0: their columns go, the later columns
+    move down."""
+    r = _copy(robot)
+    gone = set()
+    for name in links:
+        s = r["segments"][r["link_names"].index(name)]
+        gone.add(s.q_index)
+        s.joint_type, s.q_index = JOINT_FIXED, -1
+    keep = [c for c in range(robot["n_dof"]) if c not in gone]
+    col = {c: i for i, c in enumerate(keep)}
+    for s in r["segments"]:
+        if s.q_index >= 0:
+            s.q_index = col[s.q_index]
+    r.update(n_dof=len(keep), lower=[r["lower"][c] for c in keep], upper=[r["upper"][c] for c in keep])
+    return r
+
+
+def with_joint_moving(robot, link, jtype, axis, lower, upper):
+    """`robot` with the FIXED joint of segment `link` made a moving one (about / along `axis` of its frame); it takes the
+    column after the robot's."""
+    r = _copy(robot)
+    s = r["segments"][r["link_names"].index(link)]
+    assert s.joint_type == JOINT_FIXED
+    s.joint_type, s.q_index = jtype, robot["n_dof"]
+    s.axis[:] = axis
+    r.update(n_dof=robot["n_dof"] + 1, lower=r["lower"] + [lower], upper=r["upper"] + [upper])
+    return r
+
+
+def on_prismatic_axes(robot, axes):
+    """`robot` carried by a chain of prismatic axes [(name, axis, lower, upper)] from the scene root (the first carries
+    the second, the last carries the robot's root segments).  The axes take the columns after the robot's, so their
+    columns are out of segment order."""
+    n, D = len(axes), robot["n_dof"]
+    r = _copy(robot)
+    segs = [_seg(i - 1, JOINT_PRISMATIC, D + i, (0, 0, 0), ax) for i, (_, ax, _, _) in enumerate(axes)]
+    for s in r["segments"]:
+        s.parent = n - 1 if s.parent < 0 else s.parent + n
+    for sp in r["spheres"]:
+        sp.segment += n
+    r.update(n_dof=D + n, segments=segs + r["segments"], lower=r["lower"] + [a[2] for a in axes],
+             upper=r["upper"] + [a[3] for a in axes], link_names=[a[0] for a in axes] + r["link_names"],
+             tool=robot["tool"] + n)
+    if "tool_left" in robot:
+        r["tool_left"] = robot["tool_left"] + n
+    return r
+
+
+def linear_axis():
+    """1 DOF: one prismatic axis (x, +-0.8 m) 0.5 m above the floor, carrying a 0.15 m payload sphere on a 0.2 m bracket
+    and the tool frame at the payload."""
+    segs = [_seg(-1, JOINT_FIXED, -1, (0, 0, 0.5)), _seg(0, JOINT_PRISMATIC, 0, (0, 0, 0), (1, 0, 0)),
+            _seg(1, JOINT_FIXED, -1, (0, 0, -0.2))]
+    return dict(n_dof=1, segments=segs, lower=[-0.8], upper=[0.8], spheres=[_sphere(2, (0, 0, 0), 0.15)],
+                link_names=["base_link", "carriage", "payload"], tool=2)
+
+
+def scara():
+    """4 DOF SCARA (revolute z, revolute z, prismatic quill down, revolute z), a sphere on each link and one at the tool.
+    The joint columns are out of segment order: the segments in chain order hold the columns 1, 3, 0, 2."""
+    segs = [_seg(-1, JOINT_FIXED, -1, (0, 0, 0.45)),
+            _seg(0, JOINT_REVOLUTE, 1, (0, 0, 0), (0, 0, 1)),
+            _seg(1, JOINT_REVOLUTE, 3, (0.35, 0, 0), (0, 0, 1)),
+            _seg(2, JOINT_PRISMATIC, 0, (0.3, 0, 0), (0, 0, -1)),
+            _seg(3, JOINT_REVOLUTE, 2, (0, 0, -0.1), (0, 0, 1)),
+            _seg(4, JOINT_FIXED, -1, (0, 0, -0.08))]
+    spheres = [_sphere(1, (0.18, 0, 0), 0.08), _sphere(2, (0.15, 0, 0), 0.07), _sphere(3, (0, 0, 0), 0.05),
+               _sphere(5, (0, 0, 0), 0.04)]
+    return dict(n_dof=4, segments=segs, lower=[0.0, -2.5, -3.0, -2.5], upper=[0.25, 2.5, 3.0, 2.5], spheres=spheres,
+                link_names=["base_link", "link1", "link2", "quill", "flange", "tool"], tool=5)
+
+
+def pr2_arm_5dof():
+    """The PR2 right arm with r_upper_arm_roll_joint and r_forearm_roll_joint FIXED."""
+    return with_joints_fixed(pr2_arm("r"), ["r_upper_arm_roll_link", "r_forearm_roll_link"])
+
+
+def pr2_arm_on_rail():
+    """8 DOF: the PR2 right arm on a linear rail along x (+-0.5 m; column 7)."""
+    return on_prismatic_axes(pr2_arm("r"), [("rail_x", (1, 0, 0), -0.5, 0.5)])
+
+
+def pr2_arm_on_gantry():
+    """9 DOF: the PR2 right arm on an x-y gantry (x carries y, +-0.5 m each; columns 7 and 8)."""
+    return on_prismatic_axes(pr2_arm("r"), [("gantry_x", (1, 0, 0), -0.5, 0.5), ("gantry_y", (0, 1, 0), -0.5, 0.5)])
+
+
+_DUAL_FIXED = ["r_forearm_roll_link", "l_forearm_roll_link", "l_wrist_roll_link", "r_upper_arm_roll_link"]
+
+
+def pr2_dual_arm_fixed(n_fixed):
+    """14 - n_fixed DOF (1 <= n_fixed <= 4): the dual arm with the first n_fixed of both forearm rolls, the left wrist roll
+    and the right upper arm roll FIXED."""
+    return with_joints_fixed(pr2_dual_arm(), _DUAL_FIXED[:n_fixed])
+
+
+def pr2_dual_arm_on_lift(rail=False):
+    """15 DOF: the dual arm with its torso lift moving (prismatic z, 0 to 0.3 m; column 14); 16 DOF with `rail`: and the
+    whole robot on a linear rail along x (+-0.5 m; column 15)."""
+    r = with_joint_moving(pr2_dual_arm(), "torso_lift_link", JOINT_PRISMATIC, (0, 0, 1), 0.0, 0.3)
+    return on_prismatic_axes(r, [("rail_x", (1, 0, 0), -0.5, 0.5)]) if rail else r
+
+
+# The robots of this module by joint count (maker functions): every count from 1 to 16 but 3 and 6
+BY_JOINT_COUNT = {1: linear_axis, 2: spherebot, 4: scara, 5: pr2_arm_5dof, 7: pr2_arm,
+                  8: pr2_arm_on_rail, 9: pr2_arm_on_gantry, 10: lambda: pr2_dual_arm_fixed(4),
+                  11: lambda: pr2_dual_arm_fixed(3), 12: lambda: pr2_dual_arm_fixed(2),
+                  13: lambda: pr2_dual_arm_fixed(1), 14: pr2_dual_arm, 15: pr2_dual_arm_on_lift,
+                  16: lambda: pr2_dual_arm_on_lift(rail=True)}
+
+
 SPHEREBOT_OBSTACLES = np.array([[0, 0, 0, 0.5], [-0.75, 0, 0, 0.5], [0, 0.75, 0, 0.5]], dtype=np.float64)
 
 
